@@ -3,9 +3,11 @@
 //   * operands are bf16, K-major (activations [rows, K], nn.Linear weights [out, in]) or MN-major (given as [K, rows]: the
 //     weight gradient dW = dY^T X and the InfoNCE gradient), staged into shared memory by TMA with the 128-byte swizzle,
 //     BLOCK_K = 64, four pipeline stages (4 x 48 KB);
-//   * one CTA per 128 x 256 output tile, three warpgroups: warpgroup 0 issues the TMA loads (one thread, register budget
-//     lowered with setmaxnreg), warpgroups 1 and 2 own 64 rows each and issue wgmma.m64n256k16 (fp32 accumulators in
-//     registers, 128 per thread);
+//   * persistent: one CTA per SM walks 128 x 256 output tiles (grouped in bands of row panels, see kBandM) with the stage ring
+//     running on across tiles, so the next tile's loads overlap the current tile's epilogue.  Three warpgroups: in warpgroup 0
+//     one thread issues the TMA loads and warps 1-3 stage the next tile's epilogue operands (LayerNorm row statistics, column
+//     vectors) in shared memory (register budget lowered with setmaxnreg); warpgroups 1 and 2 own 64 rows each and issue
+//     wgmma.m64n256k16 (fp32 accumulators in registers, 128 per thread);
 //   * the fused epilogue runs on the accumulator fragments and stores straight to global memory.  A thread holds two rows
 //     (r, r + 8) x 2 adjacent columns of every 8-column group, so per-row reductions (LayerNorm statistics, soft-max partials)
 //     are finished with two shuffles inside a quad.
@@ -34,7 +36,19 @@ constexpr int kABytes = kBlockM * kBlockK * 2;   // 16 KB
 constexpr int kBBytes = kBlockN * kBlockK * 2;   // 32 KB
 constexpr int kStageBytes = kABytes + kBBytes;
 constexpr int kThreads = 384;
-constexpr int kSmemBytes = kStages * kStageBytes + 1024 + 1024;   // + barriers + alignment slack
+// Tiles run in bands of kBandM row panels, row panel fastest inside a band: the CTAs resident at one time cover a few A
+// panels and a run of weight panels, so each weight panel is read from HBM about once per band instead of once per row panel.
+// On an H100 bands of 8 and 16 time the same; bands of 1 (row-major tile order) make the GeGLU GEMM about 6 % slower.
+constexpr int kBandM = 8;
+
+// Epilogue operands of one tile, staged in shared memory by the spare warps of the producer warpgroup while the consumers
+// run the mainloop (two buffers: tile i + 1 is staged while tile i's epilogue reads).
+struct EpiOperands {
+  float2 row[kBlockM];   // fused-LayerNorm (mu, rstd) of the tile's rows
+  float colsum[kBlockN], bias[kBlockN], gamma[kBlockN], colscale[kBlockN];   // the tile's slices of the column vectors
+};
+constexpr int kStagerThreads = 96;   // warps 1-3 of warpgroup 0
+constexpr int kSmemBytes = kStages * kStageBytes + 1024 + 2 * sizeof(EpiOperands) + 1024;   // + barriers + alignment slack
 
 struct GemmGeom {
   int M, N, K;          // per group: rows, output columns, reduction length (= taps * kb_inner * 64 when windowed)
@@ -47,7 +61,7 @@ struct GemmGeom {
   // boxes, one per 64-wide MN chunk, 8 KB apart, and the wgmma descriptors select the transposed (MN-major) layout.
   int a_mn;
   int b_mn;
-  // Small-M split-K (gemm_bf16): the K range is cut into pieces of kb_per_piece k-blocks (0 = off); CTA (piece, tile) stores its
+  // Small-M split-K (gemm_bf16): the K range is cut into pieces of kb_per_piece k-blocks (0 = off); work unit (piece, tile) stores its
   // raw fp32 accumulators into slab `piece` of split_ws ([pieces][m_pad][N]) and gemm_split_epilogue_kernel adds the slabs in
   // piece order (deterministic) and applies the epilogue.
   int kb_per_piece;
@@ -120,7 +134,11 @@ OPB_DEVICE void wgmma_m64n256k16(float (&d)[128], uint64_t desc_a, uint64_t desc
 // ----------------------------------------------------------------------------------------------
 // kernel
 // ----------------------------------------------------------------------------------------------
-// row statistics for the fused-LayerNorm epilogue: either precomputed (mu, rstd) or reduced here from partial records
+// Row statistics for the fused-LayerNorm epilogue: either precomputed (mu, rstd) or reduced here from partial records, in
+// record order.  The variance E[x^2] - mu^2 is rounded explicitly: once (kFusedVar: the GeGLU and residual epilogues) or after
+// the product and the difference each (the others).  That is how earlier versions of this kernel evaluated it, so results
+// stay bit-identical, and they no longer depend on how the compiler contracts the expression where it is inlined.
+template <bool kFusedVar = false>
 OPB_DEVICE void load_ln_stats(const GemmEpilogue& ep, int row, int M, float& mu, float& rs) {
   mu = 0.f; rs = 1.f;
   const int rc = row < M ? row : M - 1;
@@ -132,7 +150,9 @@ OPB_DEVICE void load_ln_stats(const GemmEpilogue& ep, int row, int M, float& mu,
       s1 += v.x; s2 += v.y;
     }
     mu = s1 / ep.ln_dim;
-    rs = rsqrtf(fmaxf(s2 / ep.ln_dim - mu * mu, 0.f) + ep.ln_eps);
+    const float ex2 = s2 / ep.ln_dim;
+    const float var = kFusedVar ? fmaf(-mu, mu, ex2) : __fsub_rn(ex2, __fmul_rn(mu, mu));
+    rs = rsqrtf(fmaxf(var, 0.f) + ep.ln_eps);
   } else if (ep.ln_mu != nullptr) {
     mu = ep.ln_mu[rc];
     rs = ep.ln_rstd[rc];
@@ -155,14 +175,18 @@ OPB_DEVICE void mbar_wait_quiet(uint64_t* bar, uint32_t parity) {
   }
 }
 
+// One tile's k-blocks.  `it0` counts the k-blocks this CTA consumed for earlier tiles: the stage ring and its phases run on
+// across tiles, so the producer fills the next tile's stages while the current tile's epilogue runs.
 template <int TA, int TB>
-OPB_DEVICE void mainloop(float (&d)[128], uint8_t* smem, uint64_t* full, uint64_t* empty, int num_k_blocks, int cw) {
+OPB_DEVICE void mainloop(float (&d)[128], uint8_t* smem, uint64_t* full, uint64_t* empty, int num_k_blocks, int cw,
+                         uint32_t it0) {
   // descriptor advance per 16-deep wgmma: 32 B inside the swizzle row (K-major) or two 8-row k groups = 2048 B (MN-major)
   constexpr uint32_t step_a = TA ? 2048 : 32, step_b = TB ? 2048 : 32;
   const bool signal = (threadIdx.x & 31) == 0;
   for (int kb = 0; kb < num_k_blocks; ++kb) {
-    const int s = kb % kStages;
-    mbar_wait_quiet(&full[s], (kb / kStages) & 1);
+    const uint32_t it = it0 + kb;
+    const uint32_t s = it % kStages;
+    mbar_wait_quiet(&full[s], (it / kStages) & 1);
     const uint32_t sa = smem_u32(smem + s * kStageBytes) + cw * 8192;   // this warpgroup's 64 rows (K-major) / M chunk (MN-major)
     const uint32_t sb = smem_u32(smem + s * kStageBytes + kABytes);
     fence_acc(d);
@@ -177,21 +201,49 @@ OPB_DEVICE void mainloop(float (&d)[128], uint8_t* smem, uint64_t* full, uint64_
       wgmma_wait<1>();
       fence_acc(d);
       __syncwarp();
-      if (signal) mbar_arrive(&empty[(kb - 1) % kStages]);
+      if (signal) mbar_arrive(&empty[(it - 1) % kStages]);
     }
   }
   wgmma_wait<0>();
   fence_acc(d);
+  __syncwarp();
+  if (signal) mbar_arrive(&empty[(it0 + num_k_blocks - 1) % kStages]);
+}
+
+// the epilogues that take their operands from EpiOperands (the contrastive-head ones read none of them)
+constexpr bool epi_staged(int epi) { return epi != EPI_LSE_PARTIAL && epi != EPI_SOFTMAX_GRAD; }
+
+// Stager side: fill `st` for tile (m_blk, n_blk, grp), thread `t` of kStagerThreads.
+template <int EPI>
+OPB_DEVICE void stage_epi_operands(EpiOperands* st, const GemmEpilogue& ep, const GemmGeom& geo, int m_blk, int n_blk, int grp,
+                                   int t) {
+  if (ep.ln_partial != nullptr || ep.ln_mu != nullptr) {
+    for (int r = t; r < kBlockM; r += kStagerThreads) {
+      float mu, rs;
+      load_ln_stats<EPI == EPI_GEGLU_BF16 || EPI == EPI_RESID_F32>(ep, m_blk * kBlockM + r, geo.M, mu, rs);
+      st->row[r] = make_float2(mu, rs);
+    }
+  }
+  for (int c = t; c < kBlockN; c += kStagerThreads) {
+    const int tc = n_blk * kBlockN + c;
+    const bool ok = tc < geo.N;
+    const int col = grp * geo.N + tc;
+    st->colsum[c] = ok && ep.ln_colsum != nullptr ? ep.ln_colsum[col] : 0.f;
+    st->bias[c] = ok && ep.bias != nullptr ? ep.bias[col] : 0.f;
+    st->gamma[c] = ok && ep.gamma != nullptr ? ep.gamma[col] : 0.f;
+    st->colscale[c] = ok && ep.colscale != nullptr ? ep.colscale[col] : 0.f;
+  }
 }
 
 template <int EPI>
-OPB_DEVICE void epilogue(const float (&d)[128], const GemmEpilogue& ep, const GemmGeom& geo, int m_blk, int n_blk, int grp,
-                         int cw) {
+OPB_DEVICE void epilogue(const float (&d)[128], const GemmEpilogue& ep, const GemmGeom& geo, const EpiOperands* st, int m_blk,
+                         int n_blk, int grp, int cw) {
   const int M = geo.M, N = geo.N;
   const int t = threadIdx.x & 127;
   const int lane = t & 31;
   const int quad = lane & 3;
-  const int rbase = m_blk * kBlockM + cw * 64 + (t >> 5) * 16 + (lane >> 2);
+  const int rloc = cw * 64 + (t >> 5) * 16 + (lane >> 2);   // row inside the tile (fragment row r)
+  const int rbase = m_blk * kBlockM + rloc;
   const int col0 = n_blk * kBlockN;   // first column of the tile inside the group
   const int gcol0 = grp * N;          // first global output column of the group
 #pragma unroll
@@ -278,8 +330,8 @@ OPB_DEVICE void epilogue(const float (&d)[128], const GemmEpilogue& ep, const Ge
       gz = quad_sum(gz);
       if (row_ok && quad == 0) ep.ws[static_cast<long>(n_blk) * M + row] = gz;
     } else {
-      float mu, rs;
-      load_ln_stats(ep, row, M, mu, rs);
+      const float2 mr = (ep.ln_partial != nullptr || ep.ln_mu != nullptr) ? st->row[rloc + 8 * h] : make_float2(0.f, 1.f);
+      const float mu = mr.x, rs = mr.y;
       const bool has_ln = ep.ln_colsum != nullptr;
       float st_sum = 0.f, st_sq = 0.f;   // partial statistics of the stored values (next LayerNorm)
       if constexpr (EPI == EPI_GEGLU_BF16) {
@@ -287,16 +339,15 @@ OPB_DEVICE void epilogue(const float (&d)[128], const GemmEpilogue& ep, const Ge
 #pragma unroll
         for (int j = 0; j < 16; ++j) {
           const int tc = 8 * j + 2 * quad;    // gate column inside the tile; its linear partner is tc + 128
-          const int pc = col0 + tc;           // packed (interleaved) weight row of the gate half
           float g0 = d[4 * j + 2 * h], g1 = d[4 * j + 2 * h + 1];
           float l0 = d[4 * (j + 16) + 2 * h], l1 = d[4 * (j + 16) + 2 * h + 1];
           if (has_ln) {
-            const float2 cg = ldf2(ep.ln_colsum + pc), cl = ldf2(ep.ln_colsum + pc + kBlockN / 2);
+            const float2 cg = ldf2(st->colsum + tc), cl = ldf2(st->colsum + tc + kBlockN / 2);
             g0 = rs * (g0 - mu * cg.x); g1 = rs * (g1 - mu * cg.y);
             l0 = rs * (l0 - mu * cl.x); l1 = rs * (l1 - mu * cl.y);
           }
           if (ep.bias != nullptr) {
-            const float2 bg = ldf2(ep.bias + pc), bl = ldf2(ep.bias + pc + kBlockN / 2);
+            const float2 bg = ldf2(st->bias + tc), bl = ldf2(st->bias + tc + kBlockN / 2);
             g0 += bg.x; g1 += bg.y; l0 += bl.x; l1 += bl.y;
           }
           const float u0 = gelu_erf(g0) * l0, u1 = gelu_erf(g1) * l1;
@@ -313,21 +364,22 @@ OPB_DEVICE void epilogue(const float (&d)[128], const GemmEpilogue& ep, const Ge
       } else {
 #pragma unroll
         for (int j = 0; j < 32; ++j) {
-          const int tc = col0 + 8 * j + 2 * quad;    // column inside the group
+          const int lc = 8 * j + 2 * quad;           // column inside the tile
+          const int tc = col0 + lc;                  // column inside the group
           if (tc >= N) continue;
           const int col = gcol0 + tc;
           float x0 = d[4 * j + 2 * h], x1 = d[4 * j + 2 * h + 1];
           if (has_ln) {
-            const float2 c = ldf2(ep.ln_colsum + col);
+            const float2 c = ldf2(st->colsum + lc);
             x0 = rs * (x0 - mu * c.x); x1 = rs * (x1 - mu * c.y);
           }
           if (ep.bias != nullptr) {
-            const float2 b = ldf2(ep.bias + col);
+            const float2 b = ldf2(st->bias + lc);
             x0 += b.x; x1 += b.y;
           }
           if constexpr (EPI == EPI_STORE_BF16 || EPI == EPI_GELU_BF16) {
             if (ep.colscale != nullptr) {
-              const float2 s = ldf2(ep.colscale + col);
+              const float2 s = ldf2(st->colscale + lc);
               x0 *= s.x; x1 *= s.y;
             }
             if constexpr (EPI == EPI_GELU_BF16) { x0 = gelu_erf(x0); x1 = gelu_erf(x1); }
@@ -335,7 +387,7 @@ OPB_DEVICE void epilogue(const float (&d)[128], const GemmEpilogue& ep, const Ge
           } else {
             if constexpr (EPI == EPI_RESID_F32) {
               if (ep.gamma != nullptr) {
-                const float2 g = ldf2(ep.gamma + col);
+                const float2 g = ldf2(st->gamma + lc);
                 x0 *= g.x; x1 *= g.y;
               }
               if (ep.resid != nullptr && row_ok) {
@@ -361,6 +413,29 @@ OPB_DEVICE void epilogue(const float (&d)[128], const GemmEpilogue& ep, const Ge
   }
 }
 
+// Work unit -> tile.  Units are split-K piece-major (a single piece unless split-K), then group-major; inside a group the
+// tiles run in bands of kBandM row panels, row panel fastest.
+struct TileCoord {
+  int piece, grp, m_blk, n_blk;
+};
+OPB_DEVICE TileCoord tile_coord(int unit, int num_m_tiles, int num_n_tiles, int groups) {
+  const int per_group = num_m_tiles * num_n_tiles;
+  TileCoord c;
+  c.piece = unit / (per_group * groups);
+  const int tile = unit - c.piece * per_group * groups;
+  c.grp = tile / per_group;
+  const int tin = tile - c.grp * per_group;
+  const int band = tin / (kBandM * num_n_tiles);
+  const int m0 = band * kBandM;
+  const int band_rows = min(kBandM, num_m_tiles - m0);
+  const int r = tin - m0 * num_n_tiles;
+  c.m_blk = m0 + r % band_rows;
+  c.n_blk = r / band_rows;
+  return c;
+}
+
+// Persistent: the grid holds as many CTAs as can be resident and CTA b runs units b, b + gridDim.x, ...  Barrier set-up and
+// descriptor prefetch happen once per CTA.
 template <int EPI>
 __global__ void __launch_bounds__(kThreads, 1)
 gemm_bf16_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__ CUtensorMap tm_b, const GemmEpilogue ep,
@@ -371,21 +446,17 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant
   if ((smem_u32(smem) & 1023u) != 0) __trap();
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + kStages * kStageBytes);
   uint64_t* empty = full + kStages;
+  uint64_t* epi_full = empty + kStages;   // [2] operands of the buffer's tile are staged
+  uint64_t* epi_empty = epi_full + 2;     // [2] the buffer's epilogue is done reading
+  EpiOperands* epi_ops = reinterpret_cast<EpiOperands*>(smem + kStages * kStageBytes + 1024);
 
   const int wg = threadIdx.x >> 7;
   const int num_m_tiles = (geo.M + kBlockM - 1) / kBlockM;
   const int num_n_tiles = (geo.N + kBlockN - 1) / kBlockN;
-  const int tiles_per_group = num_m_tiles * num_n_tiles;
-  const int tiles_main = tiles_per_group * geo.groups;
-  const int piece = blockIdx.x / tiles_main;             // 0 unless split-K
-  const int tile = blockIdx.x - piece * tiles_main;
-  const int grp = tile / tiles_per_group;
-  const int tin = tile - grp * tiles_per_group;
-  const int m_blk = tin / num_n_tiles;   // n-fastest rasterisation: CTAs running together share a few A row panels (L2)
-  const int n_blk = tin % num_n_tiles;
-
-  const int kb0 = geo.kb_per_piece > 0 ? piece * geo.kb_per_piece : 0;
-  const int kb1 = geo.kb_per_piece > 0 ? min(geo.num_k_blocks, kb0 + geo.kb_per_piece) : geo.num_k_blocks;
+  const int pieces = geo.kb_per_piece > 0 ? (geo.num_k_blocks + geo.kb_per_piece - 1) / geo.kb_per_piece : 1;
+  const int units = num_m_tiles * num_n_tiles * geo.groups * pieces;
+  // split-K pieces store raw accumulators and need no epilogue operands
+  const bool staged = epi_staged(EPI) && geo.kb_per_piece == 0;
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tm_a);
@@ -394,38 +465,56 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant
       mbar_init(&full[i], 1);
       mbar_init(&empty[i], 8);   // lane 0 of each of the 8 consumer warps
     }
+    for (int i = 0; i < 2; ++i) {
+      mbar_init(&epi_full[i], kStagerThreads);
+      mbar_init(&epi_empty[i], 8);
+    }
     fence_barrier_init();
   }
   __syncthreads();
 
   if (wg == 0) {
-    // ===================== TMA producer =====================
     asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
     if (threadIdx.x == 0) {
-      const int a_row = m_blk * kBlockM;
-      const int b_row = grp * geo.b_group_rows + n_blk * kBlockN;
-      const int a_c0 = grp * geo.a_group_c0;
-      int kin = kb0 % geo.kb_inner, tap = kb0 / geo.kb_inner;
-      for (int kb = kb0; kb < kb1; ++kb) {
-        const int i = kb - kb0;
-        const int s = i % kStages;
-        mbar_wait_quiet(&empty[s], ((i / kStages) & 1) ^ 1);
-        uint8_t* sa = smem + s * kStageBytes;
-        uint8_t* sb = sa + kABytes;
-        mbar_arrive_expect_tx(&full[s], kStageBytes);     // out-of-bounds box elements are zero-filled and counted
-        if (geo.a_mn) {
+      // ===================== TMA producer =====================
+      uint32_t it = 0;   // k-blocks issued by this CTA: stage it % kStages, phase (it / kStages) & 1
+      for (int unit = blockIdx.x; unit < units; unit += gridDim.x) {
+        const TileCoord tc = tile_coord(unit, num_m_tiles, num_n_tiles, geo.groups);
+        const int kb0 = geo.kb_per_piece > 0 ? tc.piece * geo.kb_per_piece : 0;
+        const int kb1 = geo.kb_per_piece > 0 ? min(geo.num_k_blocks, kb0 + geo.kb_per_piece) : geo.num_k_blocks;
+        const int a_row = tc.m_blk * kBlockM;
+        const int b_row = tc.grp * geo.b_group_rows + tc.n_blk * kBlockN;
+        const int a_c0 = tc.grp * geo.a_group_c0;
+        int kin = kb0 % geo.kb_inner, tap = kb0 / geo.kb_inner;
+        for (int kb = kb0; kb < kb1; ++kb, ++it) {
+          const uint32_t s = it % kStages;
+          mbar_wait_quiet(&empty[s], ((it / kStages) & 1) ^ 1);
+          uint8_t* sa = smem + s * kStageBytes;
+          uint8_t* sb = sa + kABytes;
+          mbar_arrive_expect_tx(&full[s], kStageBytes);     // out-of-bounds box elements are zero-filled and counted
+          if (geo.a_mn) {
 #pragma unroll
-          for (int i = 0; i < kBlockM / 64; ++i) tma_load_2d(&tm_a, &full[s], sa + i * 8192, a_row + 64 * i, kb * kBlockK);
-        } else {
-          tma_load_3d(&tm_a, &full[s], sa, a_c0 + kin * kBlockK, tap, a_row);
-        }
-        if (geo.b_mn) {
+            for (int i = 0; i < kBlockM / 64; ++i) tma_load_2d(&tm_a, &full[s], sa + i * 8192, a_row + 64 * i, kb * kBlockK);
+          } else {
+            tma_load_3d(&tm_a, &full[s], sa, a_c0 + kin * kBlockK, tap, a_row);
+          }
+          if (geo.b_mn) {
 #pragma unroll
-          for (int i = 0; i < kBlockN / 64; ++i) tma_load_2d(&tm_b, &full[s], sb + i * 8192, b_row + 64 * i, kb * kBlockK);
-        } else {
-          tma_load_2d(&tm_b, &full[s], sb, kb * kBlockK, b_row);
+            for (int i = 0; i < kBlockN / 64; ++i) tma_load_2d(&tm_b, &full[s], sb + i * 8192, b_row + 64 * i, kb * kBlockK);
+          } else {
+            tma_load_2d(&tm_b, &full[s], sb, kb * kBlockK, b_row);
+          }
+          if (++kin == geo.kb_inner) { kin = 0; ++tap; }
         }
-        if (++kin == geo.kb_inner) { kin = 0; ++tap; }
+      }
+    } else if (threadIdx.x >= 32 && staged) {
+      // ===================== epilogue-operand stager (warps 1-3) =====================
+      uint32_t j = 0;   // tiles staged: buffer j & 1, phase (j >> 1) & 1
+      for (int unit = blockIdx.x; unit < units; unit += gridDim.x, ++j) {
+        const TileCoord tc = tile_coord(unit, num_m_tiles, num_n_tiles, geo.groups);
+        mbar_wait_quiet(&epi_empty[j & 1], ((j >> 1) & 1) ^ 1);
+        stage_epi_operands<EPI>(&epi_ops[j & 1], ep, geo, tc.m_blk, tc.n_blk, tc.grp, threadIdx.x - 32);
+        mbar_arrive(&epi_full[j & 1]);
       }
     }
   } else {
@@ -435,29 +524,41 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant
     float d[128];
 #pragma unroll
     for (int i = 0; i < 128; ++i) d[i] = 0.f;
-    if (geo.a_mn) {
-      if (geo.b_mn) mainloop<1, 1>(d, smem, full, empty, kb1 - kb0, cw);
-      else mainloop<1, 0>(d, smem, full, empty, kb1 - kb0, cw);
-    } else {
-      if (geo.b_mn) mainloop<0, 1>(d, smem, full, empty, kb1 - kb0, cw);
-      else mainloop<0, 0>(d, smem, full, empty, kb1 - kb0, cw);
-    }
-    if (geo.kb_per_piece > 0) {
-      // split-K piece: raw partial accumulators of all m_pad rows into this piece's slab (plain stores, no atomics)
-      const int t = threadIdx.x & 127, lane = t & 31;
-      const int r0 = m_blk * kBlockM + cw * 64 + (t >> 5) * 16 + (lane >> 2);
-      float* w = geo.split_ws + static_cast<long>(piece) * geo.m_pad * geo.N;
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-#pragma unroll
-        for (int j = 0; j < 32; ++j) {
-          const int col = n_blk * kBlockN + 8 * j + 2 * (lane & 3);
-          if (col < geo.N)
-            *reinterpret_cast<float2*>(w + static_cast<long>(r0 + 8 * h) * geo.N + col) = make_float2(d[4 * j + 2 * h], d[4 * j + 2 * h + 1]);
-        }
+    uint32_t it = 0, j = 0;
+    for (int unit = blockIdx.x; unit < units; unit += gridDim.x, ++j) {
+      const TileCoord tc = tile_coord(unit, num_m_tiles, num_n_tiles, geo.groups);
+      const int kb0 = geo.kb_per_piece > 0 ? tc.piece * geo.kb_per_piece : 0;
+      const int kb1 = geo.kb_per_piece > 0 ? min(geo.num_k_blocks, kb0 + geo.kb_per_piece) : geo.num_k_blocks;
+      if (geo.a_mn) {
+        if (geo.b_mn) mainloop<1, 1>(d, smem, full, empty, kb1 - kb0, cw, it);
+        else mainloop<1, 0>(d, smem, full, empty, kb1 - kb0, cw, it);
+      } else {
+        if (geo.b_mn) mainloop<0, 1>(d, smem, full, empty, kb1 - kb0, cw, it);
+        else mainloop<0, 0>(d, smem, full, empty, kb1 - kb0, cw, it);
       }
-    } else {
-      epilogue<EPI>(d, ep, geo, m_blk, n_blk, grp, cw);
+      it += kb1 - kb0;
+      if (geo.kb_per_piece > 0) {
+        // split-K piece: raw partial accumulators of all m_pad rows into this piece's slab (plain stores, no atomics)
+        const int t = threadIdx.x & 127, lane = t & 31;
+        const int r0 = tc.m_blk * kBlockM + cw * 64 + (t >> 5) * 16 + (lane >> 2);
+        float* w = geo.split_ws + static_cast<long>(tc.piece) * geo.m_pad * geo.N;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+#pragma unroll
+          for (int c = 0; c < 32; ++c) {
+            const int col = tc.n_blk * kBlockN + 8 * c + 2 * (lane & 3);
+            if (col < geo.N)
+              *reinterpret_cast<float2*>(w + static_cast<long>(r0 + 8 * h) * geo.N + col) = make_float2(d[4 * c + 2 * h], d[4 * c + 2 * h + 1]);
+          }
+        }
+      } else if (staged) {
+        mbar_wait_quiet(&epi_full[j & 1], (j >> 1) & 1);
+        epilogue<EPI>(d, ep, geo, &epi_ops[j & 1], tc.m_blk, tc.n_blk, tc.grp, cw);
+        __syncwarp();
+        if ((threadIdx.x & 31) == 0) mbar_arrive(&epi_empty[j & 1]);
+      } else {
+        epilogue<EPI>(d, ep, geo, nullptr, tc.m_blk, tc.n_blk, tc.grp, cw);
+      }
     }
   }
 }
@@ -589,15 +690,19 @@ template <int EPI>
 static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, const GemmEpilogue& ep, const GemmGeom& geo,
                        cudaStream_t stream) {
   auto kern = gemm_bf16_kernel<EPI>;
-  static bool configured = false;
-  if (!configured) {
+  static int resident = 0;   // CTAs resident at once over the whole GPU
+  if (resident == 0) {
     if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes) != cudaSuccess)
       return OPB_ERR_CUDA;
-    configured = true;
+    int per_sm = 0;
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, kThreads, kSmemBytes) != cudaSuccess || per_sm < 1)
+      return OPB_ERR_CUDA;
+    resident = per_sm * sm_count();
   }
   const int pieces = geo.kb_per_piece > 0 ? (geo.num_k_blocks + geo.kb_per_piece - 1) / geo.kb_per_piece : 1;
-  const long tiles = static_cast<long>((geo.M + kBlockM - 1) / kBlockM) * ((geo.N + kBlockN - 1) / kBlockN) * geo.groups * pieces;
-  kern<<<static_cast<unsigned>(tiles), kThreads, kSmemBytes, stream>>>(ta, tb, ep, geo);
+  const long units = static_cast<long>((geo.M + kBlockM - 1) / kBlockM) * ((geo.N + kBlockN - 1) / kBlockN) * geo.groups * pieces;
+  const unsigned grid = static_cast<unsigned>(units < resident ? units : resident);
+  kern<<<grid, kThreads, kSmemBytes, stream>>>(ta, tb, ep, geo);
   return cudaGetLastError() == cudaSuccess ? OPB_OK : OPB_ERR_CUDA;
 }
 
