@@ -133,8 +133,10 @@ def attention_tc(qkv, rp, key_pad, B, S, H, out=None, ln_stats=None, lse=None):
 
 
 def gemm_ln(a, w, epi, out, *, ln_mu=None, ln_rstd=None, ln_colsum=None, bias=None, colscale=None, gamma=None,
-            resid=None, stats_out=None, out_bf16=None, cta_group=0, workspace=None, ln_partial=None):
-    """GEMM through `opb_gemm_bf16_ex`: fused LayerNorm of the A operand (ln_*), statistics / bf16 side outputs."""
+            resid=None, stats_out=None, out_bf16=None, cta_group=0, workspace=None, ln_partial=None, out_group=0,
+            out_group_stride=0, out_row_offset=0, out_group_valid=0, resid_period=0, resid_row_offset=0):
+    """GEMM through `opb_gemm_bf16_ex`: fused LayerNorm of the A operand (ln_*), statistics / bf16 side outputs, and the
+    row remapping of `gemm`."""
     _need_cuda(a, w, out)
     assert a.dtype == torch.bfloat16 and w.dtype == torch.bfloat16 and a.stride(-1) == 1 and w.stride(1) == 1
     M, Kd = a.shape
@@ -150,6 +152,8 @@ def gemm_ln(a, w, epi, out, *, ln_mu=None, ln_rstd=None, ln_colsum=None, bias=No
     args.out_bf16 = _ptr(out_bf16) or None
     args.ldo_bf16 = out_bf16.stride(-2) if out_bf16 is not None else 0
     args.cta_group = cta_group
+    args.out_group, args.out_group_stride, args.out_row_offset = out_group, out_group_stride, out_row_offset
+    args.out_group_valid, args.resid_period, args.resid_row_offset = out_group_valid, resid_period, resid_row_offset
     if ln_partial is not None:      # (records tensor, parts, dim, eps)
         args.ln_partial, args.ln_parts, args.ln_dim, args.ln_eps = ln_partial[0].data_ptr(), ln_partial[1], ln_partial[2], ln_partial[3]
     if workspace is not None:
@@ -380,9 +384,10 @@ def split_bf16x3_x4(xs, sides):
 _TICKETS = {}
 
 
-def infonce_forward2(a3, b3, a_all3, b_all3, scale, target_offset, eps, n_valid=0):
+def infonce_forward2(a3, b3, a_all3, b_all3, scale, target_offset, eps, n_valid=0, rows=False):
     """Both directions of the InfoNCE forward in 3 launches (two LSE_PARTIAL GEMMs + one merge / reduce kernel).
-    -> (lse_a [b], lse_b [b], out3 = {loss, #correct a->b, #correct b->a})"""
+    -> (lse_a [b], lse_b [b], out3 = {loss, #correct a->b, #correct b->a}), and with `rows` also the per-row
+    losses [2 b] and arg-max columns int32 [2 b] (direction a, then b)"""
     lib = _lib.load()
     b, k = a3.shape
     n = a_all3.shape[0]
@@ -406,6 +411,8 @@ def infonce_forward2(a3, b3, a_all3, b_all3, scale, target_offset, eps, n_valid=
                                       _stream())
     _lib.check(st, "opb_infonce_merge_reduce")
     _count(3)
+    if rows:
+        return lse_a, lse_b, out3, loss_ab, am_ab
     return lse_a, lse_b, out3
 
 
