@@ -2,18 +2,24 @@
 
 The reference trains through torch autograd (transformer_layer.py:165-228, multihead_attention.py:103-126, with
 ``checkpoint_activations`` in the 4B recipes).  Here every adjoint is an sm_90a kernel behind the C-ABI
-(csrc/backward.cu, csrc/attention_bwd*.cu + the wgmma GEMM for all dX / dW products); autograd only carries the
-graph edges between five ``Function`` nodes:
+(csrc/backward.cu, csrc/attention_bwd.cu + the wgmma GEMM for all dX / dW products); autograd only carries the
+graph edges between ``Function`` nodes:
 
     TextEmbedFn / ImageEmbedFn  ->  EncoderStackFn (L layers, activations kept or recomputed)  ->  HeadFn  ->  criterion
     RelPosBiasFn (table -> dense (H,S,S_pad) bias, shared by the layers) ----^
 
+EncoderStackFn runs every encoder and decoder pass: single-modality passes (run_encoder_stack: fine-tuning, contrastive
+steps) and the concatenated 'vl' / 'al' sequences, preserve_ids student passes and the decoder of pretraining
+(run_general_stack, with the Functions of autograd_general.py around it).  Its rows are laid out by a SeqLayout, and one
+layer_forward / layer_backward pair serves both.
+
 Activation policy (keep_activations below): when the whole stack's activations fit in half of the free HBM they are KEPT (the
 training forward then runs the un-fused LayerNorm form, whose normalised operands the dW GEMMs need) and the backward is the
-adjoint only; otherwise the forward runs the inference kernels and keeps each layer's fp32 input rows, and the backward re-runs
-one layer forward per step — the reference's checkpoint_wrapper.  dW = dY^T X is an M-reduction whose operands the wgmma GEMM
-reads in place as MN-major tiles (opb_gemm_bf16_t); dX = dY W reads the forward weight the same way: nothing is transposed in
-memory.  Attention backward: csrc/attention_bwd.cu (mma.sync; S <= 224: transposed bias tables shared by the stack).
+adjoint only; otherwise the forward keeps each layer's fp32 input rows (running the inference kernels where EncoderStackFn
+allows it), and the backward re-runs one layer forward per step — the reference's checkpoint_wrapper.  dW = dY^T X is an
+M-reduction whose operands the wgmma GEMM reads in place as MN-major tiles (opb_gemm_bf16_t); dX = dY W reads the forward
+weight the same way: nothing is transposed in memory.  Attention backward: csrc/attention_bwd.cu (mma.sync; S <= 224:
+transposed bias tables shared by the stack).
 
 torch is used here for what the task calls plumbing only: allocation, dtype / layout copies (`.to`, `cat`, slicing
 `copy_`), the drop-path Bernoulli draw, and autograd's own accumulation of gradients that reach a tensor twice.
@@ -27,7 +33,8 @@ from .components import PackCache, bf16, f32
 class TrainBias:
     """Relative-position bias of a training forward: `dense` = autograd-tracked fp32 (H,S,S_pad) tensor (what the
     backward kernels read and what receives the gradient), `fast` = the same values as a kernels.RelPosBias in LUT
-    form for the attention kernel (None when S > kernels.ATTN_TC_MAX_S)."""
+    form for the attention kernel (None when S > kernels.ATTN_TC_MAX_S).  `lut` is always None, so that code reading a
+    kernels.RelPosBias sees a TrainBias as one in dense form."""
 
     def __init__(self, dense, fast=None):
         self.dense, self.fast, self.lut = dense, fast, None
@@ -69,18 +76,14 @@ def _tr(x):
     return K.transpose_bf16(xp)
 
 
-_BWD_T = __import__("os").environ.get("OPB_ATTN_BWD_T", "1") != "0"      # 0: dense bias tables in the attention backward (A/B)
-_CENTER = __import__("os").environ.get("OPB_DBIAS_CENTER", "1") != "0"   # 0: keep the accumulated bias gradient as is (A/B)
-_DW_MN = __import__("os").environ.get("OPB_DW_MN", "1") != "0"      # 0: transposed copies + K-major GEMM (round-1 path, for A/B)
-
-
 def _dw(dy, x, dtype):
     """dW [N, Kw] = dy[M, N]^T x[M, Kw]  (fp32 accumulate; stored in the parameter's dtype).  A reduction over the M rows:
-    both operands are MN-major for the tensor cores and are read in place (opb_gemm_bf16_t); no transposed copies."""
+    both operands are MN-major for the tensor cores and are read in place (opb_gemm_bf16_t) when their rows are 16-byte
+    aligned; otherwise they go through transposed copies and the K-major GEMM."""
     out = torch.empty(dy.shape[1], x.shape[1], dtype=torch.float32 if dtype == torch.float32 else torch.bfloat16,
                       device=dy.device)
     epi = K.EPI_STORE_F32 if out.dtype == torch.float32 else K.EPI_STORE_BF16
-    if _DW_MN and dy.shape[1] % 8 == 0 and x.shape[1] % 8 == 0 and dy.stride(0) % 8 == 0 and x.stride(0) % 8 == 0 \
+    if dy.shape[1] % 8 == 0 and x.shape[1] % 8 == 0 and dy.stride(0) % 8 == 0 and x.stride(0) % 8 == 0 \
             and dy.data_ptr() % 16 == 0 and x.data_ptr() % 16 == 0:
         K.gemm_t(dy, x, epi, out, a_mn=True, b_mn=True)
     else:
@@ -98,14 +101,51 @@ def _dx(dy, w, n_out, out=None):
 
 
 # ----------------------------------------------------------------------------------------------------------------
+# row layout
+# ----------------------------------------------------------------------------------------------------------------
+class SeqLayout:
+    """parts = [(modality, S_p), ...] in sequence order (text first, transformer_encoder.py:127-134).
+
+    Rows are MODALITY-MAJOR: part p owns the contiguous rows [off_p, off_p + B*S_p) of the residual stream, row =
+    off_p + b*S_p + s.  Every GEMM (shared QKV / out_proj over all rows, per-modality GeGLU / fc2 over one part's rows —
+    transformer_layer.py:210-217) then runs on a plain contiguous row range.  Only attention needs a sample's tokens
+    adjacent (batch-major rows b*S + lo_p + s): with several parts the QKV rows are permuted there and the attention output
+    back by `opb_row_gather` (two 16-byte-vector copies per layer).  A single-modality pass is one part, and both orders
+    coincide (to_bm = to_mm = None)."""
+
+    def __init__(self, B, parts, device):
+        self.B, self.parts = B, list(parts)
+        self.S = sum(s for _, s in parts)
+        self.M = B * self.S
+        self.offs, self.los = [], []
+        off = lo = 0
+        for _, s in parts:
+            self.offs.append(off)
+            self.los.append(lo)
+            off += B * s
+            lo += s
+        self.to_bm = self.to_mm = None
+        if len(parts) > 1:
+            # batch-major row (b, lo_p + s)  <-  modality-major row off_p + b * S_p + s
+            cols = []
+            for (_, s), off in zip(parts, self.offs):
+                cols.append(off + torch.arange(B, device=device)[:, None] * s + torch.arange(s, device=device)[None, :])
+            self.to_bm = torch.cat(cols, dim=1).reshape(-1).contiguous()              # [B*S]: source mm row of every bm row
+            inv = torch.empty_like(self.to_bm)
+            inv[self.to_bm] = torch.arange(self.M, device=device)
+            self.to_mm = inv.contiguous()                                             # source bm row of every mm row
+
+    def rows(self, p):
+        return slice(self.offs[p], self.offs[p] + self.B * self.parts[p][1])
+
+    def row_scale(self, per_sample):
+        """per-sample fp32 [B] -> per-row fp32 [M] in modality-major order (drop-path, transformer_layer.py:80-86)."""
+        return torch.cat([per_sample.repeat_interleave(s) for _, s in self.parts]).contiguous()
+
+
+# ----------------------------------------------------------------------------------------------------------------
 # one encoder layer
 # ----------------------------------------------------------------------------------------------------------------
-LAYER_PARAM_NAMES = ("q_proj.weight", "q_proj.bias", "k_proj.weight", "v_proj.weight", "v_proj.bias", "out_proj.weight",
-                     "out_proj.bias", "ln.weight", "ln.bias", "self_attn_layer_norm.weight", "self_attn_layer_norm.bias",
-                     "final_layer_norm.weight", "final_layer_norm.bias", "gamma_1", "gamma_2", "wi_0.weight", "wi_1.weight",
-                     "ffn_ln.weight", "ffn_ln.bias", "fc2.weight", "fc2.bias")
-
-
 def _check_structure(layer, ffn):
     a = layer.self_attn
     if a.ln is None or not isinstance(ffn[2], torch.nn.LayerNorm) or layer.attn_ln is not None or a.c_attn is not None:
@@ -114,8 +154,8 @@ def _check_structure(layer, ffn):
 
 
 def shared_params(layer):
-    """The 15 modality-shared parameters of a layer (LAYER_PARAM_NAMES[:15]); gamma_1 / gamma_2 are None when the layer was
-    built with use_layer_scale=False (the pretraining decoder, pretrain_vl_3B.yaml:168)."""
+    """The 15 modality-shared parameters of a layer, in the order layer_backward returns their gradients; gamma_1 /
+    gamma_2 are None when the layer was built with use_layer_scale=False (the pretraining decoder, pretrain_vl_3B.yaml:168)."""
     a = layer.self_attn
     return [a.q_proj.weight, a.q_proj.bias, a.k_proj.weight, a.v_proj.weight, a.v_proj.bias, a.out_proj.weight,
             a.out_proj.bias, a.ln.weight, a.ln.bias, layer.self_attn_layer_norm.weight, layer.self_attn_layer_norm.bias,
@@ -123,17 +163,10 @@ def shared_params(layer):
 
 
 def ffn_params(layer, modality):
-    """The 6 parameters of one modality's FFN (LAYER_PARAM_NAMES[15:])."""
+    """The 6 parameters of one modality's FFN, in the order layer_backward returns their gradients."""
     ffn = getattr(layer, f"{modality}_ffn")
     _check_structure(layer, ffn)
     return [ffn[0].wi_0.weight, ffn[0].wi_1.weight, ffn[2].weight, ffn[2].bias, ffn[3].weight, ffn[3].bias]
-
-
-def layer_params(layer, modality):
-    """The 21 parameters of one layer on the `modality` path, in LAYER_PARAM_NAMES order."""
-    if layer.gamma_1 is None:
-        raise NotImplementedError("single-modality fast path expects use_layer_scale (the encoder of every recipe)")
-    return shared_params(layer) + ffn_params(layer, modality)
 
 
 def shared_train_pack(layer):
@@ -169,201 +202,259 @@ def ffn_train_pack(layer, modality):
     return cache.get(ps, build)
 
 
-def layer_train_pack(layer, modality):
-    """Shared + FFN packs merged (the shared half is built once per layer, whatever number of modalities train)."""
-    return {**shared_train_pack(layer), **ffn_train_pack(layer, modality)}
-
-
-def layer_forward_train(layer, x, bias, key_pad, B, S, modality, row_scale, keep, fast_bias=None):
-    """x fp32 [M, d] -> (x_out fp32 [M, d], saved activations or None).  Un-fused LayerNorm form of
-    transformer_layer.py:165-228; `row_scale` [M] = drop-path keep mask / keep_prob (:80-86) or None."""
-    p = layer_train_pack(layer, modality)
+def layer_forward(layer, x, lay, bias, key_pad, row_scale, keep, fast_bias=None):
+    """x fp32 [M, d] (rows laid out by `lay`) -> (x_out fp32 [M, d], saved activations or None).  Un-fused LayerNorm form of
+    transformer_layer.py:165-228 with the per-modality FFN of :203-219, so every normalised operand of the dW GEMMs is in HBM.
+    bias: dense fp32 (H,S,S_pad) / (B,H,S,S_pad) or None; fast_bias: the same values as a kernels.RelPosBias in LUT form, or
+    None; key_pad uint8 (B,S) batch-major or None; row_scale [M] = drop-path keep mask / keep_prob (:80-86) or None."""
+    p = shared_train_pack(layer)
     d, F_, H = layer.embed_dim, layer.ffn_embed_dim, layer.self_attn.num_heads
-    M = B * S
+    B, S, M = lay.B, lay.S, lay.M
     dev = x.device
 
-    def e(n):
-        return torch.empty(M, n, dtype=torch.bfloat16, device=dev)
-    h1 = K.layernorm(x, p["ln1_w"], p["ln1_b"], e(d), eps=layer.self_attn_layer_norm.eps)
-    qkv = K.gemm(h1, p["wqkv"], K.EPI_STORE_BF16, e(3 * d), bias=p["bqkv"], colscale=p["qscale"])
+    def e(rows, n):
+        return torch.empty(rows, n, dtype=torch.bfloat16, device=dev)
+    h1 = K.layernorm(x, p["ln1_w"], p["ln1_b"], e(M, d), eps=layer.self_attn_layer_norm.eps)
+    qkv = K.gemm(h1, p["wqkv"], K.EPI_STORE_BF16, e(M, 3 * d), bias=p["bqkv"], colscale=p["qscale"])
+    if lay.to_bm is not None:
+        qkv = K.row_gather(qkv, lay.to_bm)
     lse = torch.empty(B * H * S, dtype=torch.float32, device=dev)
-    if fast_bias is not None:      # LUT-form bias (same table values as the dense form)
-        att = K.attention_tc(qkv, fast_bias, key_pad, B, S, H, out=e(d), lse=lse)
+    if fast_bias is not None:
+        att = K.attention_tc(qkv, fast_bias, key_pad, B, S, H, out=e(M, d), lse=lse)
     else:
-        att = K.attention(qkv, bias, key_pad, B, S, H, out=e(d), lse=lse)
-    a2 = K.layernorm(att, p["lni_w"], p["lni_b"], e(d), eps=layer.self_attn.ln.eps)
-    o = K.gemm(a2, p["wo"], K.EPI_STORE_BF16, e(d), bias=p["bo"])
+        att = K.attention(qkv, bias, key_pad, B, S, H, out=e(M, d), lse=lse)
+    att_mm = K.row_gather(att, lay.to_mm) if lay.to_mm is not None else att
+    a2 = K.layernorm(att_mm, p["lni_w"], p["lni_b"], e(M, d), eps=layer.self_attn.ln.eps)
+    o = K.gemm(a2, p["wo"], K.EPI_STORE_BF16, e(M, d), bias=p["bo"])
     x2 = K.scale_resid_fwd(x, o, p["g1"], row_scale, torch.empty_like(x))
-    h2 = K.layernorm(x2, p["ln2_w"], p["ln2_b"], e(d), eps=layer.final_layer_norm.eps)
-    gl = K.gemm(h2, p["w01"], K.EPI_STORE_BF16, e(2 * F_))
-    u = K.geglu_fwd(gl, e(F_))
-    u2 = K.layernorm(u, p["lnf_w"], p["lnf_b"], e(F_), eps=p["lnf_eps"])
-    f = K.gemm(u2, p["w2"], K.EPI_STORE_BF16, e(d), bias=p["b2"])
+    h2 = K.layernorm(x2, p["ln2_w"], p["ln2_b"], e(M, d), eps=layer.final_layer_norm.eps)
+    f = e(M, d)
+    ffn_saved = []
+    for pi, (m, _) in enumerate(lay.parts):
+        fp = ffn_train_pack(layer, m)
+        rs = lay.rows(pi)
+        n = rs.stop - rs.start
+        gl = K.gemm(h2[rs], fp["w01"], K.EPI_STORE_BF16, e(n, 2 * F_))
+        u = K.geglu_fwd(gl, e(n, F_))
+        u2 = K.layernorm(u, fp["lnf_w"], fp["lnf_b"], e(n, F_), eps=fp["lnf_eps"])
+        K.gemm(u2, fp["w2"], K.EPI_STORE_BF16, f[rs], bias=fp["b2"])
+        ffn_saved.append(dict(gl=gl, u=u, u2=u2) if keep else None)
     x3 = K.scale_resid_fwd(x2, f, p["g2"], row_scale, torch.empty_like(x))
-    saved = dict(h1=h1, qkv=qkv, lse=lse, att=att, a2=a2, o=o, x2=x2, h2=h2, gl=gl, u=u, u2=u2, f=f) if keep else None
+    saved = dict(h1=h1, qkv=qkv, lse=lse, att=att, att_mm=att_mm, a2=a2, o=o, x2=x2, h2=h2, f=f, ffn=ffn_saved) if keep else None
     return x3, saved
 
 
-def layer_backward(layer, x, s, dx, bias, dbias, key_pad, B, S, modality, row_scale, bias_t=None, dbias_t=None):
-    """Adjoint of layer_forward_train.  `dx` (fp32 [M, d]) holds dL/dx_out on entry and dL/dx_in on return (in place);
-    `dbias` (fp32 (H,S,S_pad) or None) accumulates the relative-position-bias gradient.  Returns the 21 parameter
-    gradients in LAYER_PARAM_NAMES order, in each parameter's dtype."""
-    p = layer_train_pack(layer, modality)
-    ps = layer_params(layer, modality)
+def layer_backward(layer, x, s, dx, lay, bias, dbias, key_pad, row_scale, bias_t=None, dbias_t=None):
+    """Adjoint of layer_forward.  `dx` (fp32 [M, d]) holds dL/dx_out on entry and dL/dx_in on return (in place); `dbias`
+    (shaped like `bias`, or None) accumulates the relative-position-bias gradient, or `dbias_t` does when the transposed
+    tables `bias_t` are given (S <= 224; the caller folds dbias_t back).  Returns the 15 shared_params gradients, then the 6
+    ffn_params gradients of each part, in each parameter's dtype (None for an absent gamma)."""
+    p = shared_train_pack(layer)
+    sp = shared_params(layer)
     d, F_, H = layer.embed_dim, layer.ffn_embed_dim, layer.self_attn.num_heads
-    M = B * S
+    B, S, M = lay.B, lay.S, lay.M
     dev = x.device
 
-    def e(n):
-        return torch.empty(M, n, dtype=torch.bfloat16, device=dev)
+    def e(rows, n):
+        return torch.empty(rows, n, dtype=torch.bfloat16, device=dev)
 
     def g(n):
         return torch.empty(n, dtype=torch.float32, device=dev)
-    # ---- FFN branch: x3 = x2 + rs * g2 * f ----
-    dg2, db2 = g(d), g(d)
-    df = K.scale_resid_bwd(dx, s["f"], p["g2"], row_scale, e(d), dgamma=dg2, dbias=db2)
-    dW2 = _dw(df, s["u2"], ps[19].dtype)
-    du2 = _dx(df, p["w2"], F_)
-    dlnf_w, dlnf_b = g(F_), g(F_)
-    du = K.layernorm_bwd(s["u"], du2, p["lnf_w"], p["lnf_b"], e(F_), eps=p["lnf_eps"], dgamma=dlnf_w, dbeta=dlnf_b)
-    dgl = K.geglu_bwd(s["gl"], du, e(2 * F_))
-    dW01 = _dw(dgl, s["h2"], ps[15].dtype)
-    dh2 = _dx(dgl, p["w01"], d)
+    # ---- FFN branch: x3 = x2 + rs * g2 * f, per modality on its own rows ----
+    one_part = len(lay.parts) == 1
+    dg2 = g(d) if p["g2"] is not None else None
+    db2 = g(d) if one_part else None           # one part: the fc2 bias gradient is the reduction fused into scale_resid_bwd
+    df = K.scale_resid_bwd(dx, s["f"], p["g2"], row_scale, e(M, d), dgamma=dg2, dbias=db2)
+    dh2 = e(M, d)
+    ffn_grads, ffn_ps = [], []
+    for pi, (m, _) in enumerate(lay.parts):
+        fp = ffn_train_pack(layer, m)
+        fps = ffn_params(layer, m)
+        rs = lay.rows(pi)
+        n = rs.stop - rs.start
+        fs = s["ffn"][pi]
+        dfp = df[rs]
+        db2p = db2 if one_part else K.colsum(dfp, g(d))
+        dW2 = _dw(dfp, fs["u2"], fps[4].dtype)
+        du2 = _dx(dfp, fp["w2"], F_)
+        dlnf_w, dlnf_b = g(F_), g(F_)
+        du = K.layernorm_bwd(fs["u"], du2, fp["lnf_w"], fp["lnf_b"], e(n, F_), eps=fp["lnf_eps"], dgamma=dlnf_w, dbeta=dlnf_b)
+        dgl = K.geglu_bwd(fs["gl"], du, e(n, 2 * F_))
+        dW01 = _dw(dgl, s["h2"][rs], fps[0].dtype)
+        _dx(dgl, fp["w01"], d, out=dh2[rs])
+        ffn_grads += [dW01[:F_], dW01[F_:], dlnf_w, dlnf_b, dW2, db2p]
+        ffn_ps += fps
     dln2_w, dln2_b = g(d), g(d)
     K.layernorm_bwd(s["x2"], dh2, p["ln2_w"], p["ln2_b"], dx, eps=layer.final_layer_norm.eps, accumulate=True,
                     dgamma=dln2_w, dbeta=dln2_b)                                   # dx = dL/dx2
     # ---- attention branch: x2 = x + rs * g1 * o ----
-    dg1, dbo = g(d), g(d)
-    do = K.scale_resid_bwd(dx, s["o"], p["g1"], row_scale, e(d), dgamma=dg1, dbias=dbo)
-    dWo = _dw(do, s["a2"], ps[5].dtype)
+    dg1 = g(d) if p["g1"] is not None else None
+    dbo = g(d)
+    do = K.scale_resid_bwd(dx, s["o"], p["g1"], row_scale, e(M, d), dgamma=dg1, dbias=dbo)
+    dWo = _dw(do, s["a2"], sp[5].dtype)
     da2 = _dx(do, p["wo"], d)
     dlni_w, dlni_b = g(d), g(d)
-    datt = K.layernorm_bwd(s["att"], da2, p["lni_w"], p["lni_b"], e(d), eps=layer.self_attn.ln.eps, dgamma=dlni_w,
+    datt = K.layernorm_bwd(s["att_mm"], da2, p["lni_w"], p["lni_b"], e(M, d), eps=layer.self_attn.ln.eps, dgamma=dlni_w,
                            dbeta=dlni_b)
-    if bias_t is not None:       # transposed bias tables (S <= 224); dbias_t is folded back by the caller
-        dqkv = K.attention_bwd_t(s["qkv"], s["att"], datt, bias_t, key_pad, s["lse"], e(3 * d), dbias_t, B, S, H,
+    if lay.to_bm is not None:
+        datt = K.row_gather(datt, lay.to_bm)
+    if bias_t is not None:
+        dqkv = K.attention_bwd_t(s["qkv"], s["att"], datt, bias_t, key_pad, s["lse"], e(M, 3 * d), dbias_t, B, S, H,
                                  layer.self_attn.scaling)
     else:
-        dqkv = K.attention_bwd(s["qkv"], s["att"], datt, bias, key_pad, s["lse"], e(3 * d), dbias, B, S, H,
+        dqkv = K.attention_bwd(s["qkv"], s["att"], datt, bias, key_pad, s["lse"], e(M, 3 * d), dbias, B, S, H,
                                layer.self_attn.scaling)
+    if lay.to_mm is not None:
+        dqkv = K.row_gather(dqkv, lay.to_mm)
     dbqkv = K.colsum(dqkv, g(3 * d))
-    dWqkv = _dw(dqkv, s["h1"], ps[0].dtype)
+    dWqkv = _dw(dqkv, s["h1"], sp[0].dtype)
     dh1 = _dx(dqkv, p["wqkv"], d)
     dln1_w, dln1_b = g(d), g(d)
     K.layernorm_bwd(x, dh1, p["ln1_w"], p["ln1_b"], dx, eps=layer.self_attn_layer_norm.eps, accumulate=True,
                     dgamma=dln1_w, dbeta=dln1_b)                                   # dx = dL/dx
     grads = [dWqkv[:d], dbqkv[:d], dWqkv[d:2 * d], dWqkv[2 * d:], dbqkv[2 * d:], dWo, dbo, dlni_w, dlni_b, dln1_w, dln1_b,
-             dln2_w, dln2_b, dg1, dg2, dW01[:F_], dW01[F_:], dlnf_w, dlnf_b, dW2, db2]
-    return [gr if gr.dtype == prm.dtype else gr.to(prm.dtype) for gr, prm in zip(grads, ps)]
+             dln2_w, dln2_b, dg1, dg2] + ffn_grads
+    return [None if gr is None else (gr if gr.dtype == prm.dtype else gr.to(prm.dtype)) for gr, prm in zip(grads, sp + ffn_ps)]
+
+
+# ----------------------------------------------------------------------------------------------------------------
+# the layer stack
+# ----------------------------------------------------------------------------------------------------------------
+def _pick(lst, i):
+    """The entry of layer i in a per-stack list that holds nothing, one entry for every layer, or one per layer."""
+    return None if not lst else (lst[0] if len(lst) == 1 else lst[i])
+
+
+def _b3(b):
+    """(1,H,S,S_pad) canvases are passed to the kernels as batch-shared (H,S,S_pad) tables."""
+    if b is not None and b.dim() == 4 and b.shape[0] == 1:
+        return b[0]
+    return b
 
 
 class EncoderStackFn(torch.autograd.Function):
-    """x0 [M, d] fp32 -> x_L [M, d] fp32 through all layers (transformer_encoder.py:172-188).
+    """x0 [M, d] fp32 (rows laid out by a SeqLayout) -> x_L [M, d] fp32 through all layers (transformer_encoder.py:172-188).
 
-    Forward: when no drop-path is active the layers run the inference kernels (fused-LayerNorm GEMM chain, fused
-    attention) and only each layer's input rows are kept.  Backward: per layer, recompute (un-fused form) + adjoint."""
+    meta = (lay, key_pad, need_grad, fast, shared_tables).  `fast` holds the LUT forms of the biases (TrainBias.fast) or is
+    empty.  `shared_tables` says that the biases are batch-shared (H,S,S_pad) tables of one relative-position table that
+    covers every column of the sequence, as in a single-modality pass.  Only then
+      - the forward runs the inference kernels (fused-LayerNorm GEMM chain, fused attention) when the activations are not
+        kept, no drop-path is active and every bias has a LUT form;
+      - the attention backward reads the biases from transposed half2 tables when S <= 224;
+      - the accumulated bias gradient is projected onto zero row sums.
+    The block canvases of concatenated sequences hold constant zeros between modalities, for which that projection is wrong.
+    Backward: per layer, the saved activations or a recompute (un-fused form), then the adjoint."""
 
     @staticmethod
     def forward(ctx, encoder, meta, x0, n_bias, *tensors):
-        B, S, modality, key_pad, fast = meta
+        lay, key_pad, need_grad, fast, shared_tables = meta
         biases = list(tensors[:n_bias])
         layers = list(encoder.layers)
         x = x0.contiguous()
-        xs, scales = [], []
+        scales = []
         for layer in layers:
             rs = None
-            if layer.training and layer.drop_path_prob > 0:
+            if layer.training and layer.drop_path_prob > 0 and need_grad:
                 # per-sample keep mask / keep_prob, one value per batch column (transformer_layer.py:80-86)
                 keep = 1.0 - layer.drop_path_prob
-                rs = ((torch.rand(B, device=x.device) < keep).float() / keep).repeat_interleave(S).contiguous()
+                rs = lay.row_scale((torch.rand(lay.B, device=x.device) < keep).float() / keep)
             if layer.training and layer.dropout_prob > 0:
                 raise NotImplementedError("dropout > 0 (every ONE-PEACE recipe trains with dropout 0.0)")
             scales.append(rs)
-
-        def pick(lst, i):
-            return None if not lst else (lst[0] if len(lst) == 1 else lst[i])
-        fused = all(r is None for r in scales) and all(l.fused_ln_supported() for l in layers) and \
-            (n_bias == 0 or (fast is not None and all(f is not None for f in fast)))
-        saved_all = None
-        if keep_activations(len(layers), B * S, x.shape[1], encoder.cfg.ffn_embed_dim, x.device):
-            saved_all = []
-            for i, layer in enumerate(layers):
-                xs.append(x)
-                x, saved = layer_forward_train(layer, x, pick(biases, i), key_pad, B, S, modality, scales[i], keep=True,
-                                               fast_bias=pick(fast, i))
-                saved_all.append(saved)
-        elif fused:
+        keep_all = need_grad and keep_activations(len(layers), lay.M, x.shape[1], encoder.cfg.ffn_embed_dim, x.device)
+        fused = shared_tables and not keep_all and all(r is None for r in scales) and \
+            all(l.fused_ln_supported() for l in layers) and all(f is not None for f in fast)
+        xs, saved_all = [], ([] if keep_all else None)
+        if fused:
             from .transformer.transformer_layer import TransformerEncoderLayer
-            d = x.shape[1]
             rows = x.clone()                      # the fused path updates the residual stream in place
-            ws = TransformerEncoderLayer.fused_workspace(B * S, d, encoder.cfg.ffn_embed_dim, encoder.num_attention_heads, x.device)
+            ws = TransformerEncoderLayer.fused_workspace(lay.M, x.shape[1], encoder.cfg.ffn_embed_dim,
+                                                         encoder.num_attention_heads, x.device)
             K.row_stats_cast(rows, ws["xb"], ws["mu"], ws["rstd"], eps=layers[0].self_attn_layer_norm.eps)
             ln1 = dict(ln_mu=ws["mu"], ln_rstd=ws["rstd"])
             for i, layer in enumerate(layers):
                 xs.append(rows.clone())
-                ln1 = layer.forward_rows_fused(rows, ws["xb"], ln1, ws, pick(fast, i), key_pad, B, S, modality)
+                ln1 = layer.forward_rows_fused(rows, ws["xb"], ln1, ws, _pick(fast, i), key_pad, lay.B, lay.S, lay.parts[0][0])
             x = rows
         else:
             for i, layer in enumerate(layers):
-                xs.append(x)
-                x, _ = layer_forward_train(layer, x, pick(biases, i), key_pad, B, S, modality, scales[i], keep=False,
-                                           fast_bias=pick(fast, i))
-        ctx.encoder, ctx.meta, ctx.n_bias = encoder, meta, n_bias
+                if need_grad:
+                    xs.append(x)
+                x, saved = layer_forward(layer, x, lay, _b3(_pick(biases, i)), key_pad, scales[i], keep_all, _pick(fast, i))
+                if keep_all:
+                    saved_all.append(saved)
+        ctx.encoder, ctx.meta = encoder, meta
         ctx.xs, ctx.scales, ctx.biases, ctx.saved_all = xs, scales, biases, saved_all
         return x
 
     @staticmethod
     def backward(ctx, grad_out):
-        B, S, modality, key_pad, fast = ctx.meta
+        lay, key_pad, _, fast, shared_tables = ctx.meta
         layers = list(ctx.encoder.layers)
-        n_bias, biases = ctx.n_bias, ctx.biases
+        biases = ctx.biases
         dx = grad_out.to(torch.float32).contiguous().clone()
         dbiases = [torch.zeros_like(b) for b in biases]
         # S <= 224: the attention backward reads the batch-shared bias from a transposed half2 table and accumulates its
         # gradient in a transposed fp32 table shared by every layer that uses the same bias; both conversions run once per stack
         bias_ts, dbias_ts = [], []
-        if biases and S <= K.BIAS_T_Q and all(b.dim() == 3 for b in biases) and _BWD_T:
+        if shared_tables and biases and lay.S <= K.BIAS_T_Q and all(b.dim() == 3 for b in biases):
             bias_ts = [K.relpos_bias_transpose(b) for b in biases]
             dbias_ts = [torch.zeros(b.shape[0], K.BIAS_T_KEYS, K.BIAS_T_Q, dtype=torch.float32, device=b.device) for b in biases]
-
-        def pick(lst, i):
-            return None if not lst else (lst[0] if len(lst) == 1 else lst[i])
         grads = [None] * len(layers)
         for i in reversed(range(len(layers))):
             layer = layers[i]
-            bias, dbias = pick(biases, i), pick(dbiases, i)
+            bias, dbias = _b3(_pick(biases, i)), _b3(_pick(dbiases, i))
             if ctx.saved_all is not None:
                 saved, ctx.saved_all[i] = ctx.saved_all[i], None
             else:
-                _, saved = layer_forward_train(layer, ctx.xs[i], bias, key_pad, B, S, modality, ctx.scales[i], keep=True,
-                                               fast_bias=pick(fast, i))
-            grads[i] = layer_backward(layer, ctx.xs[i], saved, dx, bias, dbias, key_pad, B, S, modality, ctx.scales[i],
-                                      bias_t=pick(bias_ts, i), dbias_t=pick(dbias_ts, i))
+                _, saved = layer_forward(layer, ctx.xs[i], lay, bias, key_pad, ctx.scales[i], True, _pick(fast, i))
+            grads[i] = layer_backward(layer, ctx.xs[i], saved, dx, lay, bias, dbias, key_pad, ctx.scales[i],
+                                      _pick(bias_ts, i), _pick(dbias_ts, i))
             ctx.xs[i] = None
             del saved
         for dt, db in zip(dbias_ts, dbiases):
             K.relpos_dbias_fold(dt, db)
-        if _CENTER:
-            # zero-row-sum projection of the bias gradient (csrc/attention_bwd_tc.cu: relpos_dbias_center_kernel).  Padded keys carry
-            # dS = 0, so every sample's row sums to zero over all S columns and so does the batch sum.
+        if shared_tables:
+            # zero-row-sum projection of the bias gradient (csrc/attention_bwd.cu: relpos_dbias_center_kernel).  Padded keys
+            # carry dS = 0, so every sample's row sums to zero over all S columns and so does the batch sum.
             for db in dbiases:
-                if db.dim() == 3:
-                    K.relpos_dbias_center(db)
+                K.relpos_dbias_center(db)
         flat = [g for lg in grads for g in lg]
         return (None, None, dx, None, *dbiases, *flat)
 
 
+def _stack_params(encoder, lay):
+    """Per layer: the 15 shared parameters, then the 6 FFN parameters of each part (EncoderStackFn's gradient order)."""
+    params = []
+    for layer in encoder.layers:
+        params += shared_params(layer)
+        for m, _ in lay.parts:
+            params += ffn_params(layer, m)
+    return params
+
+
 def run_encoder_stack(encoder, x, bias_list, key_pad, modality):
-    """x fp32 [B, S, d] (autograd-tracked) -> fp32 [B, S, d]."""
+    """Single-modality pass: x fp32 [B, S, d] (autograd-tracked) -> fp32 [B, S, d].  bias_list: TrainBias or dense fp32
+    (H,S,S_pad) tensors (len 0, 1 or L)."""
     B, S, d = x.shape
-    params = [p for layer in encoder.layers for p in layer_params(layer, modality)]
+    if any(layer.gamma_1 is None for layer in encoder.layers):
+        raise NotImplementedError("single-modality fast path expects use_layer_scale (the encoder of every recipe)")
+    lay = SeqLayout(B, [(modality, S)], x.device)
+    params = _stack_params(encoder, lay)
     tb = list(bias_list) if bias_list else []
     biases = [b.dense if isinstance(b, TrainBias) else b for b in tb]
     fast = [b.fast if isinstance(b, TrainBias) else None for b in tb]
     if any(not torch.is_tensor(b) for b in biases):
         raise RuntimeError("training needs the dense relative-position bias (adapters' forward_train provides it)")
-    out = EncoderStackFn.apply(encoder, (B, S, modality, key_pad, fast), x.reshape(B * S, d), len(biases), *biases, *params)
+    out = EncoderStackFn.apply(encoder, (lay, key_pad, True, fast, True), x.reshape(B * S, d), len(biases), *biases, *params)
     return out.view(B, S, d)
+
+
+def run_general_stack(encoder, x_mm, lay, key_pad, biases, need_grad):
+    """Concatenated sequences, preserve_ids student passes and the decoder: x_mm fp32 [M, d] modality-major -> fp32 [M, d].
+    biases: list (len 0, 1 or L) of dense fp32 (Bb,H,S,S_pad) canvases (autograd_general.BlockBiasFn)."""
+    return EncoderStackFn.apply(encoder, (lay, key_pad, need_grad, [], False), x_mm, len(biases), *biases,
+                                *_stack_params(encoder, lay))
 
 
 # ----------------------------------------------------------------------------------------------------------------

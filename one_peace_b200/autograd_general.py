@@ -1,244 +1,14 @@
-"""Pretraining path (SURVEY.md 8f rows 1-2): concatenated 'vl' / 'al' encoders with per-modality FFN row groups,
-preserve_ids gathers with sample-dependent relative-position bias, the mask-token canvas of the decoder, nn.Linear
-with a hand-written backward, and the DCL loss — all as ``torch.autograd.Function`` nodes whose forward AND backward
-are sm_90a kernels behind the C-ABI (the reference relies on torch autograd for every one of them).
-
-Row layout of a concatenated batch: MODALITY-MAJOR.  Part p (modality m_p, S_p tokens per sample) owns the contiguous
-rows [off_p, off_p + B*S_p) of the residual stream, row = off_p + b*S_p + s.  Every GEMM (shared QKV / out_proj over
-all rows, per-modality GeGLU / fc2 over one part's rows — transformer_layer.py:210-217) then runs on a plain
-contiguous row range.  Only attention needs a sample's tokens adjacent (batch-major rows b*S + lo_p + s): the QKV
-rows are permuted there and the attention output back by `opb_row_gather` (two 16-byte-vector copies per layer).
-
-The un-fused LayerNorm form of the layer is used (LayerNorm kernels + plain GEMM epilogues), exactly like the recompute
-of the single-modality training path (autograd.py), because every normalised operand is needed in HBM for the dW GEMMs.
+"""Pretraining path (SURVEY.md 8f rows 1-2) around the layer stack (autograd.run_general_stack): the block-diagonal
+relative-position bias canvas of concatenated 'vl' / 'al' sequences with sample-dependent preserve_ids gathers, row
+gathers (preserve_ids, the mask-token canvas of the decoder), padded-row zeroing, nn.Linear, the per-modality final
+LayerNorm and the DCL loss — all as ``torch.autograd.Function`` nodes whose forward AND backward are sm_90a kernels behind
+the C-ABI (the reference relies on torch autograd for every one of them).
 """
 import torch
 
 from . import kernels as K
-from .autograd import _dw, _dx, ffn_params, ffn_train_pack, keep_activations, shared_params, shared_train_pack
+from .autograd import _dw, _dx
 from .components import bf16, f32
-
-
-# ----------------------------------------------------------------------------------------------------------------
-# layout
-# ----------------------------------------------------------------------------------------------------------------
-class SeqLayout:
-    """parts = [(modality, S_p), ...] in sequence order (text first, transformer_encoder.py:127-134)."""
-
-    def __init__(self, B, parts, device):
-        self.B, self.parts = B, list(parts)
-        self.S = sum(s for _, s in parts)
-        self.M = B * self.S
-        self.offs, self.los = [], []
-        off = lo = 0
-        for _, s in parts:
-            self.offs.append(off)
-            self.los.append(lo)
-            off += B * s
-            lo += s
-        self.to_bm = self.to_mm = None
-        if len(parts) > 1:
-            # batch-major row (b, lo_p + s)  <-  modality-major row off_p + b * S_p + s
-            cols = []
-            for (_, s), off in zip(parts, self.offs):
-                cols.append(off + torch.arange(B, device=device)[:, None] * s + torch.arange(s, device=device)[None, :])
-            self.to_bm = torch.cat(cols, dim=1).reshape(-1).contiguous()              # [B*S]: source mm row of every bm row
-            inv = torch.empty_like(self.to_bm)
-            inv[self.to_bm] = torch.arange(self.M, device=device)
-            self.to_mm = inv.contiguous()                                             # source bm row of every mm row
-
-    def rows(self, p):
-        return slice(self.offs[p], self.offs[p] + self.B * self.parts[p][1])
-
-    def row_scale(self, per_sample):
-        """per-sample fp32 [B] -> per-row fp32 [M] in modality-major order (drop-path, transformer_layer.py:80-86)."""
-        return torch.cat([per_sample.repeat_interleave(s) for _, s in self.parts]).contiguous()
-
-
-# ----------------------------------------------------------------------------------------------------------------
-# one layer, general form
-# ----------------------------------------------------------------------------------------------------------------
-def layer_forward_general(layer, x, bias, key_pad, lay, row_scale, keep):
-    """x fp32 [M, d] (modality-major) -> (x_out, saved).  bias: dense fp32 (H,S,S_pad) / (B,H,S,S_pad) / None;
-    key_pad uint8 (B,S) batch-major or None.  transformer_layer.py:165-228 with the per-modality FFN of :203-219."""
-    p = shared_train_pack(layer)
-    d, F_, H = layer.embed_dim, layer.ffn_embed_dim, layer.self_attn.num_heads
-    B, S, M = lay.B, lay.S, lay.M
-    dev = x.device
-
-    def e(rows, n):
-        return torch.empty(rows, n, dtype=torch.bfloat16, device=dev)
-    h1 = K.layernorm(x, p["ln1_w"], p["ln1_b"], e(M, d), eps=layer.self_attn_layer_norm.eps)
-    qkv = K.gemm(h1, p["wqkv"], K.EPI_STORE_BF16, e(M, 3 * d), bias=p["bqkv"], colscale=p["qscale"])
-    if lay.to_bm is not None:
-        qkv = K.row_gather(qkv, lay.to_bm)
-    lse = torch.empty(B * H * S, dtype=torch.float32, device=dev)
-    att = K.attention(qkv, bias, key_pad, B, S, H, out=e(M, d), lse=lse)
-    att_mm = K.row_gather(att, lay.to_mm) if lay.to_mm is not None else att
-    a2 = K.layernorm(att_mm, p["lni_w"], p["lni_b"], e(M, d), eps=layer.self_attn.ln.eps)
-    o = K.gemm(a2, p["wo"], K.EPI_STORE_BF16, e(M, d), bias=p["bo"])
-    x2 = K.scale_resid_fwd(x, o, p["g1"], row_scale, torch.empty_like(x))
-    h2 = K.layernorm(x2, p["ln2_w"], p["ln2_b"], e(M, d), eps=layer.final_layer_norm.eps)
-    f = e(M, d)
-    ffn_saved = []
-    for pi, (m, _) in enumerate(lay.parts):
-        fp = ffn_train_pack(layer, m)
-        rs = lay.rows(pi)
-        n = rs.stop - rs.start
-        gl = K.gemm(h2[rs], fp["w01"], K.EPI_STORE_BF16, e(n, 2 * F_))
-        u = K.geglu_fwd(gl, e(n, F_))
-        u2 = K.layernorm(u, fp["lnf_w"], fp["lnf_b"], e(n, F_), eps=fp["lnf_eps"])
-        K.gemm(u2, fp["w2"], K.EPI_STORE_BF16, f[rs], bias=fp["b2"])
-        ffn_saved.append(dict(gl=gl, u=u, u2=u2) if keep else None)
-    x3 = K.scale_resid_fwd(x2, f, p["g2"], row_scale, torch.empty_like(x))
-    saved = dict(h1=h1, qkv=qkv, lse=lse, att=att, att_mm=att_mm, a2=a2, o=o, x2=x2, h2=h2, f=f, ffn=ffn_saved) if keep else None
-    return x3, saved
-
-
-def layer_backward_general(layer, x, s, dx, bias, dbias, key_pad, lay, row_scale):
-    """Adjoint of layer_forward_general; `dx` fp32 [M, d] in place.  Returns (15 shared grads, [6 FFN grads per part])."""
-    p = shared_train_pack(layer)
-    sp = shared_params(layer)
-    d, F_, H = layer.embed_dim, layer.ffn_embed_dim, layer.self_attn.num_heads
-    B, S, M = lay.B, lay.S, lay.M
-    dev = x.device
-
-    def e(rows, n):
-        return torch.empty(rows, n, dtype=torch.bfloat16, device=dev)
-
-    def g(n):
-        return torch.empty(n, dtype=torch.float32, device=dev)
-    # ---- FFN branch: x3 = x2 + rs * g2 * f, per modality on its own rows ----
-    dg2 = g(d) if p["g2"] is not None else None
-    df = K.scale_resid_bwd(dx, s["f"], p["g2"], row_scale, e(M, d), dgamma=dg2)
-    dh2 = e(M, d)
-    ffn_grads = []
-    for pi, (m, _) in enumerate(lay.parts):
-        fp = ffn_train_pack(layer, m)
-        fps = ffn_params(layer, m)
-        rs = lay.rows(pi)
-        n = rs.stop - rs.start
-        fs = s["ffn"][pi]
-        dfp = df[rs]
-        db2 = K.colsum(dfp, g(d))
-        dW2 = _dw(dfp, fs["u2"], fps[4].dtype)
-        du2 = _dx(dfp, fp["w2"], F_)
-        dlnf_w, dlnf_b = g(F_), g(F_)
-        du = K.layernorm_bwd(fs["u"], du2, fp["lnf_w"], fp["lnf_b"], e(n, F_), eps=fp["lnf_eps"], dgamma=dlnf_w, dbeta=dlnf_b)
-        dgl = K.geglu_bwd(fs["gl"], du, e(n, 2 * F_))
-        dW01 = _dw(dgl, s["h2"][rs], fps[0].dtype)
-        _dx(dgl, fp["w01"], d, out=dh2[rs])
-        grads = [dW01[:F_], dW01[F_:], dlnf_w, dlnf_b, dW2, db2]
-        ffn_grads.append([gr if gr.dtype == prm.dtype else gr.to(prm.dtype) for gr, prm in zip(grads, fps)])
-    dln2_w, dln2_b = g(d), g(d)
-    K.layernorm_bwd(s["x2"], dh2, p["ln2_w"], p["ln2_b"], dx, eps=layer.final_layer_norm.eps, accumulate=True,
-                    dgamma=dln2_w, dbeta=dln2_b)                                   # dx = dL/dx2
-    # ---- attention branch: x2 = x + rs * g1 * o ----
-    dg1 = g(d) if p["g1"] is not None else None
-    dbo = g(d)
-    do = K.scale_resid_bwd(dx, s["o"], p["g1"], row_scale, e(M, d), dgamma=dg1, dbias=dbo)
-    dWo = _dw(do, s["a2"], sp[5].dtype)
-    da2 = _dx(do, p["wo"], d)
-    dlni_w, dlni_b = g(d), g(d)
-    datt = K.layernorm_bwd(s["att_mm"], da2, p["lni_w"], p["lni_b"], e(M, d), eps=layer.self_attn.ln.eps, dgamma=dlni_w,
-                           dbeta=dlni_b)
-    if lay.to_bm is not None:
-        datt = K.row_gather(datt, lay.to_bm)
-    dqkv = K.attention_bwd(s["qkv"], s["att"], datt, bias, key_pad, s["lse"], e(M, 3 * d), dbias, B, S, H,
-                           layer.self_attn.scaling)
-    if lay.to_mm is not None:
-        dqkv = K.row_gather(dqkv, lay.to_mm)
-    dbqkv = K.colsum(dqkv, g(3 * d))
-    dWqkv = _dw(dqkv, s["h1"], sp[0].dtype)
-    dh1 = _dx(dqkv, p["wqkv"], d)
-    dln1_w, dln1_b = g(d), g(d)
-    K.layernorm_bwd(x, dh1, p["ln1_w"], p["ln1_b"], dx, eps=layer.self_attn_layer_norm.eps, accumulate=True,
-                    dgamma=dln1_w, dbeta=dln1_b)                                   # dx = dL/dx
-    grads = [dWqkv[:d], dbqkv[:d], dWqkv[d:2 * d], dWqkv[2 * d:], dbqkv[2 * d:], dWo, dbo, dlni_w, dlni_b, dln1_w, dln1_b,
-             dln2_w, dln2_b, dg1, dg2]
-    shared = [None if (gr is None or prm is None) else (gr if gr.dtype == prm.dtype else gr.to(prm.dtype))
-              for gr, prm in zip(grads, sp)]
-    return shared, ffn_grads
-
-
-class GeneralStackFn(torch.autograd.Function):
-    """x0 [M, d] fp32 (modality-major) -> x_L through all layers (transformer_encoder.py:172-188), activation recompute
-    per layer in the backward like the reference's checkpoint_wrapper (one_peace_pretrain.py:83-91)."""
-
-    @staticmethod
-    def forward(ctx, encoder, meta, x0, n_bias, *tensors):
-        lay, key_pad, need_grad = meta
-        biases = list(tensors[:n_bias])
-        layers = list(encoder.layers)
-        x = x0.contiguous()
-        xs, scales = [], []
-        keep_all = need_grad and keep_activations(len(layers), x.shape[0], x.shape[1], encoder.cfg.ffn_embed_dim, x.device)
-        saved_all = [] if keep_all else None
-
-        def pick(lst, i):
-            return None if not lst else (lst[0] if len(lst) == 1 else lst[i])
-        for i, layer in enumerate(layers):
-            rs = None
-            if layer.training and layer.drop_path_prob > 0 and need_grad:
-                keep = 1.0 - layer.drop_path_prob
-                rs = lay.row_scale((torch.rand(lay.B, device=x.device) < keep).float() / keep)
-            if layer.training and layer.dropout_prob > 0:
-                raise NotImplementedError("dropout > 0 (every ONE-PEACE recipe trains with dropout 0.0)")
-            scales.append(rs)
-            if need_grad:
-                xs.append(x)
-            b = pick(biases, i)
-            x, saved = layer_forward_general(layer, x, _b3(b), key_pad, lay, rs, keep=keep_all)
-            if keep_all:
-                saved_all.append(saved)
-        ctx.encoder, ctx.meta, ctx.n_bias = encoder, meta, n_bias
-        ctx.xs, ctx.scales, ctx.biases, ctx.saved_all = xs, scales, biases, saved_all
-        return x
-
-    @staticmethod
-    def backward(ctx, grad_out):
-        lay, key_pad, _ = ctx.meta
-        layers = list(ctx.encoder.layers)
-        biases = ctx.biases
-        dx = grad_out.to(torch.float32).contiguous().clone()
-        dbiases = [torch.zeros_like(b) for b in biases]
-
-        def pick(lst, i):
-            return None if not lst else (lst[0] if len(lst) == 1 else lst[i])
-        shared, ffns = [None] * len(layers), [None] * len(layers)
-        for i in reversed(range(len(layers))):
-            layer = layers[i]
-            bias, dbias = _b3(pick(biases, i)), _b3(pick(dbiases, i))
-            if ctx.saved_all is not None:
-                saved, ctx.saved_all[i] = ctx.saved_all[i], None
-            else:
-                _, saved = layer_forward_general(layer, ctx.xs[i], bias, key_pad, lay, ctx.scales[i], keep=True)
-            shared[i], ffns[i] = layer_backward_general(layer, ctx.xs[i], saved, dx, bias, dbias, key_pad, lay, ctx.scales[i])
-            ctx.xs[i] = None
-            del saved
-        flat = []
-        for i in range(len(layers)):
-            flat += shared[i]
-            for fg in ffns[i]:
-                flat += fg
-        return (None, None, dx, None, *dbiases, *flat)
-
-
-def _b3(b):
-    """(1,H,S,S_pad) canvases are passed to the kernels as batch-shared (H,S,S_pad) tables."""
-    if b is not None and b.dim() == 4 and b.shape[0] == 1:
-        return b[0]
-    return b
-
-
-def run_general_stack(encoder, x_mm, lay, key_pad, biases, need_grad):
-    """x_mm fp32 [M, d] modality-major -> fp32 [M, d].  biases: list (len 0, 1 or L) of dense fp32 canvases."""
-    params = []
-    for layer in encoder.layers:
-        params += shared_params(layer)
-        for m, _ in lay.parts:
-            params += ffn_params(layer, m)
-    return GeneralStackFn.apply(encoder, (lay, key_pad, need_grad), x_mm, len(biases), *biases, *params)
 
 
 # ----------------------------------------------------------------------------------------------------------------

@@ -9,7 +9,7 @@ recipe, pretrain_vl_3B.yaml:151-168) with the mask-token canvas, the three contr
     model(..., *_preserve_ids=..., encoder_type=...)                 -> decoder features at every position    (:136-161)
 
 Every arithmetic step is an sm_90a kernel behind the C-ABI, forward and backward (one_peace_b200/autograd.py for the
-single-modality encoder passes, autograd_general.py for concatenated sequences, preserve_ids gathers and the decoder).
+encoder and decoder layer stacks, autograd_general.py for the bias canvases, preserve_ids gathers, linears and the DCL loss).
 """
 import math
 from dataclasses import dataclass

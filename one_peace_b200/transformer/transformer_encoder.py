@@ -75,8 +75,9 @@ class TransformerEncoder(FairseqEncoder):
         """General encoder forward (transformer_encoder.py:73-232) for concatenated modalities ('vl' / 'al'), preserve_ids
         student passes and the decoder.  parts = [(modality, x fp32 (B,S_p,d), pad uint8 (B,S_p) or None, bias source or None)]
         in sequence order.  Returns ([features fp32 (B,S_p,d) per part, after that modality's final LayerNorm], [pad per part]).
-        Differentiable end to end (one_peace_b200/autograd_general.py)."""
-        from ..autograd_general import BlockBiasFn, FinalNormFn, SeqLayout, ZeroPadFn, run_general_stack
+        Differentiable end to end (one_peace_b200/autograd.py, autograd_general.py)."""
+        from ..autograd import SeqLayout, run_general_stack
+        from ..autograd_general import BlockBiasFn, FinalNormFn, ZeroPadFn
         B, d = parts[0][1].shape[0], parts[0][1].shape[2]
         dev = parts[0][1].device
         H = self.num_attention_heads

@@ -8,7 +8,7 @@ import synth
 
 
 def test_seq_layout_permutations_are_inverse_and_ordered():
-    from one_peace_b200.autograd_general import SeqLayout
+    from one_peace_b200.autograd import SeqLayout
     B, parts = 3, [("text", 5), ("image", 7)]
     lay = SeqLayout(B, parts, "cpu")
     assert lay.S == 12 and lay.M == 36 and lay.offs == [0, 15] and lay.los == [0, 5]
