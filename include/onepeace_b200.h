@@ -104,7 +104,8 @@ int opb_attention_fwd(const void* qkv, const float* bias, const uint8_t* key_pad
  * rows [0, seg_split) and [seg_split, S); the bias is block-diagonal (zero between modalities, :148-158).
  * lut_max fp32 [H] = max_l lut[h][l] (for seg_split > 0: max(that, 0)): the kernel shifts the soft-max by the upper bound
  * max_j q.k_j + lut_max[h] of the biased row maximum, so the row maximum is found without touching the bias.
- * Returns OPB_ERR_UNSUPPORTED for S > 384 or LUT + codes larger than 16 KB (callers then use opb_attention_fwd).
+ * Any S and lut_len: the kernel reads the LUT from global memory.  The adapters choose this form for S <= 384 and
+ * opb_attention_fwd with the dense table above that.
  */
 int opb_attention_tc_fwd(const void* qkv, const float* lut, const float* lut_max, int lut_len, const int32_t* code_row,
                          const int32_t* code_col, const uint8_t* key_pad, void* out, float* lse, float* ln_stats, int B,

@@ -159,7 +159,7 @@ class AudioAdapter(torch.nn.Module):
         return out
 
     def get_rel_pos_bias(self, seq_len):
-        """One RelPosBias per table: LUT form for the attention kernel when S <= 768, dense (H,S,S_pad) otherwise."""
+        """One RelPosBias per table: LUT form for the attention kernel when S <= 384 (kernels.ATTN_TC_MAX_S), dense (H,S,S_pad) otherwise."""
         p = self._pack()
         if not hasattr(self, "_lut_cache"):
             self._lut_cache = relpos.LutCache()

@@ -104,7 +104,7 @@ class ImageAdapter(torch.nn.Module):
         return self._pos_cache[window_size]
 
     def get_rel_pos_bias(self, seq_len):
-        """One RelPosBias per table: LUT form for the attention kernel when S <= 768, dense (H,S,S_pad) otherwise."""
+        """One RelPosBias per table: LUT form for the attention kernel when S <= 384 (kernels.ATTN_TC_MAX_S), dense (H,S,S_pad) otherwise."""
         p = self._pack()
         if not hasattr(self, "_lut_cache"):
             self._lut_cache = relpos.LutCache()
@@ -213,7 +213,7 @@ class ImageAdapter(torch.nn.Module):
                                self.cls_embedding)
         bias = None
         if self.rel_pos_table_list is not None:
-            fast = self.get_rel_pos_bias(S)            # LUT form for the attention kernel (S <= 768), same values
+            fast = self.get_rel_pos_bias(S)            # LUT form for the attention kernel (S <= 384), same values
             bias = [TrainBias(RelPosBiasFn.apply(t.weight, self.rp_bucket, S, self.attention_heads),
                               f if f.lut is not None else None) for t, f in zip(self.rel_pos_table_list, fast)]
         return x, None, bias

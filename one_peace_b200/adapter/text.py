@@ -85,7 +85,7 @@ class TextAdapter(torch.nn.Module):
         return self._cache.get(ps, build)
 
     def get_rel_pos_bias(self, seq_len):
-        """One RelPosBias per table: LUT form for the attention kernel when S <= 768, dense (H,S,S_pad) otherwise."""
+        """One RelPosBias per table: LUT form for the attention kernel when S <= 384 (kernels.ATTN_TC_MAX_S), dense (H,S,S_pad) otherwise."""
         p = self._pack()
         if not hasattr(self, "_lut_cache"):
             self._lut_cache = relpos.LutCache()
@@ -159,7 +159,7 @@ class TextAdapter(torch.nn.Module):
         bias = None
         if self.rel_pos_table_list is not None:
             S = src_tokens.size(1) + 1
-            fast = self.get_rel_pos_bias(S)            # LUT form for the attention kernel (S <= 768), same values
+            fast = self.get_rel_pos_bias(S)            # LUT form for the attention kernel (S <= 384), same values
             bias = [TrainBias(RelPosBiasFn.apply(t.weight, self.rp_bucket, S, self.attention_heads),
                               f if f.lut is not None else None) for t, f in zip(self.rel_pos_table_list, fast)]
         return x, pad, bias

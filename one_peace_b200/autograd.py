@@ -14,9 +14,10 @@ steps) and the concatenated 'vl' / 'al' sequences, preserve_ids student passes a
 layer_forward / layer_backward pair serves both.
 
 Activation policy (keep_activations below): when the whole stack's activations fit in half of the free HBM they are KEPT (the
-training forward then runs the un-fused LayerNorm form, whose normalised operands the dW GEMMs need) and the backward is the
-adjoint only; otherwise the forward keeps each layer's fp32 input rows (running the inference kernels where EncoderStackFn
-allows it), and the backward re-runs one layer forward per step — the reference's checkpoint_wrapper.  dW = dY^T X is an
+training forward then runs layer_forward, the un-fused LayerNorm form, whose normalised operands the dW GEMMs need) and the
+backward is the adjoint only; otherwise the forward keeps each layer's fp32 input rows, running the fused-LayerNorm loop of
+inference (TransformerEncoder.run_fused) where EncoderStackFn allows it and layer_forward elsewhere, and the backward
+re-runs layer_forward for one layer at a time before its adjoint — the reference's checkpoint_wrapper.  dW = dY^T X is an
 M-reduction whose operands the wgmma GEMM reads in place as MN-major tiles (opb_gemm_bf16_t); dX = dY W reads the forward
 weight the same way: nothing is transposed in memory.  Attention backward: csrc/attention_bwd.cu (mma.sync; S <= 224:
 transposed bias tables shared by the stack).
@@ -146,13 +147,6 @@ class SeqLayout:
 # ----------------------------------------------------------------------------------------------------------------
 # one encoder layer
 # ----------------------------------------------------------------------------------------------------------------
-def _check_structure(layer, ffn):
-    a = layer.self_attn
-    if a.ln is None or not isinstance(ffn[2], torch.nn.LayerNorm) or layer.attn_ln is not None or a.c_attn is not None:
-        raise NotImplementedError("the backward pass is built for the 4B layer structure (magneto_scale_attn, scale_fc on; "
-                                  "scale_attn, scale_heads off — finetune_3B.yaml:114-132)")
-
-
 def shared_params(layer):
     """The 15 modality-shared parameters of a layer, in the order layer_backward returns their gradients; gamma_1 /
     gamma_2 are None when the layer was built with use_layer_scale=False (the pretraining decoder, pretrain_vl_3B.yaml:168)."""
@@ -165,7 +159,7 @@ def shared_params(layer):
 def ffn_params(layer, modality):
     """The 6 parameters of one modality's FFN, in the order layer_backward returns their gradients."""
     ffn = getattr(layer, f"{modality}_ffn")
-    _check_structure(layer, ffn)
+    layer.check_structure()
     return [ffn[0].wi_0.weight, ffn[0].wi_1.weight, ffn[2].weight, ffn[2].bias, ffn[3].weight, ffn[3].bias]
 
 
@@ -338,7 +332,7 @@ class EncoderStackFn(torch.autograd.Function):
     meta = (lay, key_pad, need_grad, fast, shared_tables).  `fast` holds the LUT forms of the biases (TrainBias.fast) or is
     empty.  `shared_tables` says that the biases are batch-shared (H,S,S_pad) tables of one relative-position table that
     covers every column of the sequence, as in a single-modality pass.  Only then
-      - the forward runs the inference kernels (fused-LayerNorm GEMM chain, fused attention) when the activations are not
+      - the forward runs the fused-LayerNorm loop of inference (TransformerEncoder.run_fused) when the activations are not
         kept, no drop-path is active and every bias has a LUT form;
       - the attention backward reads the biases from transposed half2 tables when S <= 224;
       - the accumulated bias gradient is projected onto zero row sums.
@@ -362,20 +356,11 @@ class EncoderStackFn(torch.autograd.Function):
                 raise NotImplementedError("dropout > 0 (every ONE-PEACE recipe trains with dropout 0.0)")
             scales.append(rs)
         keep_all = need_grad and keep_activations(len(layers), lay.M, x.shape[1], encoder.cfg.ffn_embed_dim, x.device)
-        fused = shared_tables and not keep_all and all(r is None for r in scales) and \
-            all(l.fused_ln_supported() for l in layers) and all(f is not None for f in fast)
+        fused = shared_tables and not keep_all and all(r is None for r in scales) and all(f is not None for f in fast)
         xs, saved_all = [], ([] if keep_all else None)
         if fused:
-            from .transformer.transformer_layer import TransformerEncoderLayer
-            rows = x.clone()                      # the fused path updates the residual stream in place
-            ws = TransformerEncoderLayer.fused_workspace(lay.M, x.shape[1], encoder.cfg.ffn_embed_dim,
-                                                         encoder.num_attention_heads, x.device)
-            K.row_stats_cast(rows, ws["xb"], ws["mu"], ws["rstd"], eps=layers[0].self_attn_layer_norm.eps)
-            ln1 = dict(ln_mu=ws["mu"], ln_rstd=ws["rstd"])
-            for i, layer in enumerate(layers):
-                xs.append(rows.clone())
-                ln1 = layer.forward_rows_fused(rows, ws["xb"], ln1, ws, _pick(fast, i), key_pad, lay.B, lay.S, lay.parts[0][0])
-            x = rows
+            # run_fused updates the residual stream in place: x0 stays untouched
+            x = encoder.run_fused(x.clone(), fast, key_pad, lay.B, lay.S, lay.parts[0][0], inputs=xs)
         else:
             for i, layer in enumerate(layers):
                 if need_grad:

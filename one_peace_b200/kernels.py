@@ -74,7 +74,7 @@ def gemm(a, w, epi, out, *, bias=None, colscale=None, gamma=None, resid=None, ou
 
 class RelPosBias:
     """Relative-position bias of one forward in both forms the attention kernels take: the dense fp32 (H,S,S_pad)
-    table (mma.sync kernel, any S) and the LUT form (S <= 768)."""
+    table (mma.sync kernel, any S) and the LUT form (same kernel; the adapters build it for S <= ATTN_TC_MAX_S)."""
 
     def __init__(self, dense=None, lut=None, code_row=None, code_col=None, seg_split=0):
         self.dense, self.lut, self.code_row, self.code_col, self.seg_split = dense, lut, code_row, code_col, seg_split
@@ -110,13 +110,13 @@ def relpos_lut_build(table, idx):
 
 
 # LUT-form bias: the attention kernel gathers each score's bias from a per-head LUT instead of reading the dense (H,S,S_pad)
-# table.  The adapters build the LUT form for S <= 384 (OPB_ATTN_LONG_TC=1: S <= 768) and the dense table above that.
-ATTN_TC_MAX_S = 768 if __import__("os").environ.get("OPB_ATTN_LONG_TC", "0") == "1" else 384
+# table.  The adapters build the LUT form for S <= 384 and the dense table above that.
+ATTN_TC_MAX_S = 384
 
 
 def attention_tc(qkv, rp, key_pad, B, S, H, out=None, ln_stats=None, lse=None):
-    """attention with the LUT-form bias (S <= 768).  rp: RelPosBias with the LUT form (rp.seg_split > 0: two concatenated modalities,
-    block-diagonal bias; S <= 384 then)."""
+    """attention with the LUT-form bias (any S; the kernel reads the LUT from global memory).  rp: RelPosBias with the LUT form
+    (rp.seg_split > 0: two concatenated modalities, block-diagonal bias; S <= 384 then)."""
     D = H * 64
     assert qkv.dtype == torch.bfloat16 and qkv.shape == (B * S, 3 * D) and qkv.is_contiguous()
     if out is None:

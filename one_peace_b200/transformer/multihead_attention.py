@@ -1,16 +1,16 @@
 """Drop-in for the reference ``MultiheadAttention`` (models/transformer/multihead_attention.py:29-126).
 
 Same constructor arguments and parameter names (q_proj / k_proj (no bias) / v_proj / out_proj / ln /
-c_attn).  The arithmetic is three sm_90a kernels: one TMA+wgmma GEMM for the concatenated QKV
-projection (bias and the post-bias q scaling fused in the epilogue, :103-107), the fused
-bias+softmax+PV attention kernel (:108-115) and — owned by the enclosing layer, because it fuses the
-LayerScale + residual — the out_proj GEMM (:124).
+c_attn).  The module holds the parameters and launches the fused bias+softmax+PV attention kernel
+(:108-115, `run_attention`).  The QKV and out_proj GEMMs (:103-107, :124), with the LayerNorms folded into
+them, are issued by the enclosing layer (TransformerEncoderLayer.forward_rows_fused) and by the training
+forward (autograd.layer_forward).
 """
 import torch
 import torch.nn as nn
 
 from .. import kernels as K
-from ..components import LayerNorm, Linear, PackCache, bf16, f32
+from ..components import LayerNorm, Linear
 
 
 class MultiheadAttention(nn.Module):
@@ -30,43 +30,11 @@ class MultiheadAttention(nn.Module):
         self.v_proj = Linear(embed_dim, embed_dim, bias=True)
         self.q_proj = Linear(embed_dim, embed_dim, bias=True)
         self.out_proj = Linear(embed_dim, embed_dim, bias=True)
-        self._cache = PackCache()
-
-    def pack(self):
-        """bf16 [3d, d] QKV weight, fp32 bias (k has none) and the per-column q scale."""
-        def build():
-            d = self.embed_dim
-            dev = self.q_proj.weight.device
-            w = torch.cat([bf16(self.q_proj.weight), bf16(self.k_proj.weight), bf16(self.v_proj.weight)], 0).contiguous()
-            b = torch.cat([f32(self.q_proj.bias), torch.zeros(d, device=dev), f32(self.v_proj.bias)]).contiguous()
-            s = torch.ones(3 * d, device=dev)
-            s[:d] = self.scaling
-            out = dict(wqkv=w, bqkv=b, qscale=s, wo=bf16(self.out_proj.weight), bo=f32(self.out_proj.bias))
-            if self.ln is not None:
-                out["ln_w"], out["ln_b"] = f32(self.ln.weight), f32(self.ln.bias)
-            return out
-        ps = [self.q_proj.weight, self.q_proj.bias, self.k_proj.weight, self.v_proj.weight, self.v_proj.bias,
-              self.out_proj.weight, self.out_proj.bias] + ([self.ln.weight, self.ln.bias] if self.ln is not None else [])
-        return self._cache.get(ps, build)
 
     def run_attention(self, qkv, bias, key_pad, B, S, out=None, ln_stats=None, lse=None):
-        """bias: kernels.RelPosBias (or None).  the bias in LUT form (S <= 768) or as a dense table; mma.sync either way."""
+        """bias: kernels.RelPosBias (or None), in LUT form (the adapters build it for S <= kernels.ATTN_TC_MAX_S) or as a
+        dense table; mma.sync either way."""
         if bias is not None and bias.lut is not None:
             return K.attention_tc(qkv, bias, key_pad, B, S, self.num_heads, out=out, ln_stats=ln_stats, lse=lse)
         dense = bias.dense if bias is not None else None
         return K.attention(qkv, dense, key_pad, B, S, self.num_heads, out=out, ln_stats=ln_stats, lse=lse)
-
-    def attend(self, h, bias, key_pad, B, S):
-        """h: bf16 [B*S, d] (already layer-normed).  Returns the pre-out_proj tensor (after the inner LN), bf16."""
-        if self.c_attn is not None:
-            raise NotImplementedError("scale_heads=True is not used by any ONE-PEACE config (finetune_3B.yaml:130)")
-        if self.training and self.dropout_p > 0:
-            raise NotImplementedError("attention dropout is 0 in every ONE-PEACE config")
-        p = self.pack()
-        d = self.embed_dim
-        qkv = torch.empty(B * S, 3 * d, dtype=torch.bfloat16, device=h.device)
-        K.gemm(h, p["wqkv"], K.EPI_STORE_BF16, qkv, bias=p["bqkv"], colscale=p["qscale"])
-        o = self.run_attention(qkv, bias, key_pad, B, S)
-        if self.ln is not None:
-            K.layernorm(o, p["ln_w"], p["ln_b"], o, eps=self.ln.eps)
-        return o

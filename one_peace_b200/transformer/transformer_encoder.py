@@ -5,12 +5,11 @@ the reference signature (text_info / image_info / audio_info tuples from the ada
 the tuples carry the fp32 residual stream (B,S,d), a uint8/bool padding mask (or None) and the
 batch-shared (H,S,S_pad) bias table instead of the reference's expanded (B,H,S,S) tensor.
 """
-import os
-
 import torch
 import torch.nn as nn
 
 from .. import kernels as K
+from ..autograd import _pick
 from ..components import LayerNorm, PackCache, f32
 from ..fairseq_compat import FairseqEncoder
 from .transformer_layer import TransformerEncoderLayer
@@ -44,6 +43,8 @@ class TransformerEncoder(FairseqEncoder):
         if encoder_type not in ("text", "image", "audio"):
             # 'vl' / 'al' (concatenated sequences with per-modality FFN) belong to the pretraining path
             raise NotImplementedError(f"encoder_type={encoder_type!r}: only single-modality encoders are built")
+        for layer in self.layers:
+            layer.check_structure()
         x, pad, bias_list = info
         B, S, d = x.shape
         x = x.contiguous()
@@ -55,21 +56,23 @@ class TransformerEncoder(FairseqEncoder):
             # (H,S,S_pad) tensors here
             from ..autograd import run_encoder_stack
             return run_encoder_stack(self, x, bias_list, key_pad, encoder_type), pad
-        rows = x.view(B * S, d)
-        fused = os.environ.get("OPB_FUSED_LN", "1") != "0" and all(l.fused_ln_supported() for l in self.layers)
-        if fused:
-            ws = TransformerEncoderLayer.fused_workspace(B * S, d, self.cfg.ffn_embed_dim, self.num_attention_heads, x.device)
-            K.row_stats_cast(rows, ws["xb"], ws["mu"], ws["rstd"], eps=self.layers[0].self_attn_layer_norm.eps)
-            ln1 = dict(ln_mu=ws["mu"], ln_rstd=ws["rstd"])
-        for idx, layer in enumerate(self.layers):
-            bias = None
-            if bias_list:
-                bias = bias_list[0] if len(bias_list) == 1 else bias_list[idx]
-            if fused:
-                ln1 = layer.forward_rows_fused(rows, ws["xb"], ln1, ws, bias, key_pad, B, S, encoder_type)
-            else:
-                layer.forward_rows(rows, bias, key_pad, B, S, encoder_type)
+        self.run_fused(x.view(B * S, d), bias_list, key_pad, B, S, encoder_type)
         return x, pad
+
+    def run_fused(self, rows, biases, key_pad, B, S, modality, inputs=None):
+        """The fused-LayerNorm layer loop (TransformerEncoderLayer.forward_rows_fused) of a single-modality sequence.
+        rows: fp32 [B*S, d] residual stream, updated in place and returned.  biases: 0, 1 or L kernels.RelPosBias.
+        inputs: None, or a list to which a copy of each layer's input rows is appended (the recompute backward of
+        autograd.EncoderStackFn starts from them)."""
+        ws = TransformerEncoderLayer.fused_workspace(B * S, rows.shape[1], self.cfg.ffn_embed_dim, self.num_attention_heads,
+                                                     rows.device)
+        K.row_stats_cast(rows, ws["xb"], ws["mu"], ws["rstd"], eps=self.layers[0].self_attn_layer_norm.eps)
+        ln1 = dict(ln_mu=ws["mu"], ln_rstd=ws["rstd"])
+        for i, layer in enumerate(self.layers):
+            if inputs is not None:
+                inputs.append(rows.clone())
+            ln1 = layer.forward_rows_fused(rows, ws["xb"], ln1, ws, _pick(biases, i), key_pad, B, S, modality)
+        return rows
 
     def forward_general(self, parts):
         """General encoder forward (transformer_encoder.py:73-232) for concatenated modalities ('vl' / 'al'), preserve_ids

@@ -1,17 +1,17 @@
 """Drop-in for ``TransformerEncoderLayer`` / ``GeGLU`` (models/transformer/transformer_layer.py:54-228).
 
 Parameter names match the reference (self_attn.*, self_attn_layer_norm, {text,image,audio}_ffn.{0.wi_0,
-0.wi_1,2,3}, final_layer_norm, gamma_1, gamma_2).  One layer forward = 4 wgmma GEMMs + 1 attention
-kernel + 4 LayerNorm kernels; the residual stream stays fp32 in HBM and is updated in place by the
-out_proj / fc2 GEMM epilogues (gamma * (acc + bias) + residual — `fused_dropout_res`, :70-88, eval mode).
+0.wi_1,2,3}, final_layer_norm, gamma_1, gamma_2).  One layer forward (forward_rows_fused) = 4 wgmma GEMMs
++ 1 attention kernel: each of the four LayerNorms is folded into the GEMM that reads its output, with the row
+statistics taken from the epilogue of the kernel that wrote the rows.  The residual stream stays fp32 in HBM and is
+updated in place by the out_proj / fc2 GEMM epilogues (gamma * (acc + bias) + residual — `fused_dropout_res`, :70-88,
+eval mode).  The training forward that keeps the normalised activations is autograd.layer_forward.
 """
-import os
-
 import torch
 import torch.nn as nn
 
 from .. import kernels as K
-from ..components import LayerNorm, Linear, PackCache, bf16, f32
+from ..components import LayerNorm, Linear, PackCache, f32
 from .multihead_attention import MultiheadAttention
 
 
@@ -22,14 +22,6 @@ class GeGLU(nn.Module):
         super().__init__()
         self.wi_0 = Linear(embed_dim, ffn_dim, bias=False)
         self.wi_1 = Linear(embed_dim, ffn_dim, bias=False)
-
-
-def interleave_geglu(w0, w1):
-    """[F,d],[F,d] -> bf16 [2F,d] where each 256-row GEMM tile holds 128 rows of wi_0 followed by the matching
-    128 rows of wi_1, so the epilogue can form gelu(a) * b inside one accumulator tile."""
-    F_, d = w0.shape
-    assert F_ % 128 == 0, "ffn_embed_dim must be a multiple of 128"
-    return torch.stack([bf16(w0).view(F_ // 128, 128, d), bf16(w1).view(F_ // 128, 128, d)], dim=1).reshape(2 * F_, d).contiguous()
 
 
 class TransformerEncoderLayer(nn.Module):
@@ -64,40 +56,19 @@ class TransformerEncoderLayer(nn.Module):
                              LayerNorm(self.ffn_embed_dim) if cfg.scale_fc else nn.Identity(),
                              Linear(self.ffn_embed_dim, self.embed_dim))
 
-    def _ffn_pack(self, modality):
-        ffn = getattr(self, f"{modality}_ffn")
-        cache = self._cache.setdefault(modality, PackCache())
-        has_ln = isinstance(ffn[2], nn.LayerNorm)
-        ps = [ffn[0].wi_0.weight, ffn[0].wi_1.weight, ffn[3].weight, ffn[3].bias] + ([ffn[2].weight, ffn[2].bias] if has_ln else [])
-
-        def build():
-            out = dict(w01=interleave_geglu(ffn[0].wi_0.weight, ffn[0].wi_1.weight), w2=bf16(ffn[3].weight), b2=f32(ffn[3].bias))
-            if has_ln:
-                out["ln_w"], out["ln_b"] = f32(ffn[2].weight), f32(ffn[2].bias)
-            return out
-        return cache.get(ps, build)
-
-    def _norm_pack(self):
-        cache = self._cache.setdefault("_norm", PackCache())
-        ps = [self.self_attn_layer_norm.weight, self.self_attn_layer_norm.bias, self.final_layer_norm.weight,
-              self.final_layer_norm.bias] + ([self.gamma_1, self.gamma_2] if self.gamma_1 is not None else [])
-
-        def build():
-            out = dict(ln1_w=f32(ps[0]), ln1_b=f32(ps[1]), ln2_w=f32(ps[2]), ln2_b=f32(ps[3]))
-            if self.gamma_1 is not None:
-                out["g1"], out["g2"] = f32(self.gamma_1), f32(self.gamma_2)
-            return out
-        return cache.get(ps, build)
+    def check_structure(self):
+        """The forward and backward kernels are built for the layer structure of the recipes; any other raises."""
+        ffn_ok = all(isinstance(getattr(self, f"{m}_ffn")[2], nn.LayerNorm) for m in ("text", "image", "audio")
+                     if hasattr(self, f"{m}_ffn"))
+        if self.self_attn.ln is None or not ffn_ok or self.attn_ln is not None or self.self_attn.c_attn is not None:
+            raise NotImplementedError("the encoder layer is built for the 4B layer structure (magneto_scale_attn, scale_fc on; "
+                                      "scale_attn, scale_heads off — finetune_3B.yaml:114-132)")
 
     # ------------------------------------------------------------------------------------------------
     # fused-LayerNorm path: the four LayerNorms of the layer never run as kernels.  Each GEMM consumes the
     # UN-normalised bf16 rows and applies  rstd * (acc - mu * colsum) + bias'  in its epilogue (gemm.h); the row
     # statistics come from the epilogue of the kernel that produced those rows.
     # ------------------------------------------------------------------------------------------------
-    def fused_ln_supported(self):
-        ffn_ok = all(isinstance(getattr(self, f"{m}_ffn")[2], nn.LayerNorm) for m in ("text", "image", "audio")
-                     if hasattr(self, f"{m}_ffn"))
-        return self.self_attn.ln is not None and ffn_ok and self.attn_ln is None and self.self_attn.c_attn is None
 
     @staticmethod
     def _fold(weights, ln, biases, interleave=False):
@@ -166,7 +137,6 @@ class TransformerEncoderLayer(nn.Module):
         if self.training and (self.dropout_prob > 0 or self.drop_path_prob > 0):
             raise NotImplementedError("training-time dropout / drop-path: backward pass is not built yet")
         d, F_, H = self.embed_dim, self.ffn_embed_dim, self.self_attn.num_heads
-        M = B * S
         a = self._fused_attn_pack()
         f = self._fused_ffn_pack(modality)
         n_t = (d + 255) // 256
@@ -179,19 +149,13 @@ class TransformerEncoderLayer(nn.Module):
         K.gemm_ln(ws["o"], a["wo"], K.EPI_RESID_F32, x, ln_partial=(ws["part_a"], H, d, self.self_attn.ln.eps),
                   ln_colsum=a["co"], bias=a["do"], gamma=a["g1"], resid=x, stats_out=ws["part_b"], out_bf16=xb,
                   workspace=ws["tail"])
-        # LN2 -> GeGLU; emits u and the partial statistics for the FFN LayerNorm (96 records / row: reduced by a kernel)
+        # LN2 -> GeGLU; emits u and the partial statistics for the FFN LayerNorm (96 records / row, reduced in the fc2 epilogue)
         K.gemm_ln(xb, f["w01"], K.EPI_GEGLU_BF16, ws["u"], ln_partial=(ws["part_b"], n_t, d, self.final_layer_norm.eps),
                   ln_colsum=f["c01"], bias=f["d01"], stats_out=ws["part_c"])
-        # FFN LN -> fc2 -> LayerScale + residual; emits x, xb and the partial statistics for the next layer's LN1.
-        # OPB_FC2_INLINE_STATS=0 restores the separate ln_stats_finalize launch (96 records / row) for A/B runs.
+        # FFN LN -> fc2 -> LayerScale + residual; emits x, xb and the partial statistics for the next layer's LN1
         n_rec = 2 * ((2 * F_) // 256)                                                                     # 2 records / tile
-        if os.environ.get("OPB_FC2_INLINE_STATS", "1") != "0":
-            ln_ffn = dict(ln_partial=(ws["part_c"], n_rec, F_, f["lnf_eps"]))
-        else:
-            K.ln_stats_finalize(ws["part_c"], n_rec, M, F_, f["lnf_eps"], ws["mu2"], ws["rstd2"])
-            ln_ffn = dict(ln_mu=ws["mu2"], ln_rstd=ws["rstd2"])
-        K.gemm_ln(ws["u"], f["w2"], K.EPI_RESID_F32, x, ln_colsum=f["c2"], bias=f["d2"], gamma=f["g2"], resid=x,
-                  stats_out=ws["part_d"], out_bf16=xb, workspace=ws["tail"], **ln_ffn)
+        K.gemm_ln(ws["u"], f["w2"], K.EPI_RESID_F32, x, ln_partial=(ws["part_c"], n_rec, F_, f["lnf_eps"]), ln_colsum=f["c2"],
+                  bias=f["d2"], gamma=f["g2"], resid=x, stats_out=ws["part_d"], out_bf16=xb, workspace=ws["tail"])
         return dict(ln_partial=(ws["part_d"], n_t, d, self.self_attn_layer_norm.eps))
 
     @staticmethod
@@ -202,30 +166,4 @@ class TransformerEncoderLayer(nn.Module):
         return dict(qkv=e(M, 3 * d), o=e(M, d), u=e(M, F_), xb=e(M, d), part_a=e(H * M * 2, dt=f32),
                     part_b=e(n_t * M * 2, dt=f32), part_c=e(2 * ((2 * F_) // 256) * M * 2, dt=f32), part_d=e(n_t * M * 2, dt=f32),
                     tail=e(16 * 256 * d, dt=torch.float32),      # split-K slabs of the small-M GEMMs: one fp32 [M rounded up to 128, N] slab per piece
-                    mu=e(M, dt=torch.float32), rstd=e(M, dt=torch.float32), mu2=e(M, dt=torch.float32),
-                    rstd2=e(M, dt=torch.float32))
-
-    def forward_rows(self, x, bias, key_pad, B, S, modality):
-        """x: fp32 [B*S, d] residual stream, updated IN PLACE.  Single-modality sequence
-        (encoder_type in text|image|audio; transformer_layer.py:203-209)."""
-        if self.attn_ln is not None:
-            raise NotImplementedError("scale_attn=True is not used by the 4B config (finetune_3B.yaml:128)")
-        if self.training and (self.dropout_prob > 0 or self.drop_path_prob > 0):
-            raise NotImplementedError("training-time dropout / drop-path: backward pass is not built yet")
-        d, F_ = self.embed_dim, self.ffn_embed_dim
-        M = B * S
-        n = self._norm_pack()
-        a = self.self_attn.pack()
-        f = self._ffn_pack(modality)
-        dev = x.device
-        h = torch.empty(M, d, dtype=torch.bfloat16, device=dev)
-        K.layernorm(x, n["ln1_w"], n["ln1_b"], h, eps=self.self_attn_layer_norm.eps)
-        o = self.self_attn.attend(h, bias, key_pad, B, S)
-        K.gemm(o, a["wo"], K.EPI_RESID_F32, x, bias=a["bo"], gamma=n.get("g1"), resid=x)
-        K.layernorm(x, n["ln2_w"], n["ln2_b"], h, eps=self.final_layer_norm.eps)
-        u = torch.empty(M, F_, dtype=torch.bfloat16, device=dev)
-        K.gemm(h, f["w01"], K.EPI_GEGLU_BF16, u)
-        if "ln_w" in f:
-            K.layernorm(u, f["ln_w"], f["ln_b"], u, eps=getattr(self, f"{modality}_ffn")[2].eps)
-        K.gemm(u, f["w2"], K.EPI_RESID_F32, x, bias=f["b2"], gamma=n.get("g2"), resid=x)
-        return x
+                    mu=e(M, dt=torch.float32), rstd=e(M, dt=torch.float32))

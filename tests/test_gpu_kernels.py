@@ -18,6 +18,14 @@ def relerr(a, b):
     return ((a.float() - b.float()).abs().max() / (b.float().abs().max() + 1e-9)).item()
 
 
+def interleave_geglu(w0, w1):
+    """[F,d],[F,d] -> bf16 [2F,d] where each 256-row GEMM tile holds 128 rows of wi_0 followed by the matching
+    128 rows of wi_1, so the epilogue can form gelu(a) * b inside one accumulator tile."""
+    F_, d = w0.shape
+    assert F_ % 128 == 0, "ffn_embed_dim must be a multiple of 128"
+    return torch.stack([w0.bfloat16().view(F_ // 128, 128, d), w1.bfloat16().view(F_ // 128, 128, d)], dim=1).reshape(2 * F_, d).contiguous()
+
+
 @pytest.mark.parametrize("cg", [1, 2])
 @pytest.mark.parametrize("M,N,Kd", [(128, 256, 64), (1000, 384, 48), (1576, 1536, 1536), (12608, 4608, 1536), (37, 768, 256)])
 def test_gemm_store(K, cg, M, N, Kd):
@@ -36,13 +44,13 @@ def test_gemm_store(K, cg, M, N, Kd):
 
 
 @pytest.mark.parametrize("cg", [1, 2])
-def test_gemm_geglu_and_residual(K, cg):
-    M, d, F = 1000, 256, 1024
+@pytest.mark.parametrize("M", [1000, 136])           # 136: the small-batch text rows (8 x 17), one partial row panel
+def test_gemm_geglu_and_residual(K, cg, M):
+    d, F = 256, 1024
     g = torch.Generator(device="cuda").manual_seed(7)
     h = (torch.randn(M, d, device="cuda", generator=g)).bfloat16()
     w0 = (torch.randn(F, d, device="cuda", generator=g) * 0.05)
     w1 = (torch.randn(F, d, device="cuda", generator=g) * 0.05)
-    from one_peace_b200.transformer.transformer_layer import interleave_geglu
     w01 = interleave_geglu(w0, w1)
     u = torch.empty(M, F, device="cuda", dtype=torch.bfloat16)
     K.gemm(h, w01, K.EPI_GEGLU_BF16, u, cta_group=cg)

@@ -50,6 +50,17 @@ def test_forward_without_cuda_fails_loudly():
         model(src_tokens=tok, encoder_type="text")
 
 
+def test_unbuilt_layer_structure_raises_in_inference():
+    """A layer structure no recipe builds (here scale_fc off) is refused before any kernel runs, as in training."""
+    model = build("text", synth.make_state_dict(**TINY, modalities=("text",), seed=2))
+    fm = model.encoder_wrapper.fusion_model
+    for layer in fm.layers:
+        layer.text_ffn[2] = torch.nn.Identity()
+    x = torch.randn(2, 8, TINY["embed_dim"])
+    with torch.no_grad(), pytest.raises(NotImplementedError):
+        fm.run_layers((x, None, None), "text")
+
+
 def test_adam_chunk_tables_are_cached_by_shape():
     """optim/adam.py `_Table`: the chunk tables of the multi-tensor kernels depend on the tensor SIZES only — a re-allocated .grad
     (new pointer, same shape) must cost one record upload, not a rebuild of the 184 k-chunk tables (that rebuild was 0.3 ms of host
