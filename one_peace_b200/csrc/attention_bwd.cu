@@ -480,14 +480,15 @@ int attention_bwd(const void* qkv, const void* out, const void* d_out, const flo
   if (B <= 0 || S <= 0 || H <= 0 || lse == nullptr || delta == nullptr) return OPB_ERR_INVALID;
   if (bias != nullptr && (s_pad < S || (s_pad & 3))) return OPB_ERR_INVALID;
   if (dbias != nullptr && bias == nullptr) return OPB_ERR_INVALID;
-  int rc = attn_delta(d_out, out, delta, B, S, H, stream);
-  if (rc != OPB_OK) return rc;
+  // every check before the first launch: a rejected call launches nothing
   BiasT bt;
   if (bias == nullptr && dbias == nullptr) {
     if ((bias_t != nullptr || dbias_t != nullptr) && S > kTQ) return OPB_ERR_UNSUPPORTED;
     bt.bias_t = reinterpret_cast<const uint32_t*>(bias_t);
     bt.dbias_t = dbias_t;
   }
+  int rc = attn_delta(d_out, out, delta, B, S, H, stream);
+  if (rc != OPB_OK) return rc;
   static bool configured = false;
   if (!configured) {
     if (cudaFuncSetAttribute(attention_bwd_dq_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,

@@ -1,5 +1,6 @@
-"""fp64 references of the GEMM epilogues (csrc/gemm_wgmma.cu) and of the contrastive-head reductions (csrc/infonce.cu),
-with an error bound for every output element, and NaN-canary output buffers.
+"""fp64 references of the GEMM epilogues (csrc/gemm_wgmma.cu), of the contrastive-head reductions (csrc/infonce.cu) and of
+the attention forward and backward (csrc/attention.cu, csrc/attention_bwd.cu), with an error bound for every output
+element, and NaN-canary output buffers.
 
 Plain PyTorch on whatever device the inputs live on; nothing here calls the extension.
 
@@ -24,6 +25,39 @@ A kernel output ``got`` passes ``assert_within`` when, element by element,
           records (``ln_stats_ref``) and, for the contrastive head, the errors of the bf16x3 logits.
 ``u_out`` 2^-8 for a bf16 output, 0 for fp32.  Round-to-nearest to 8 significant bits moves the kernel's fp32 value v by
           less than 2^-8 |v|, and |v| exceeds |ref| by at most the fp32 error (itself far inside tau * mag).
+
+Attention (``attention_ref``, ``attention_bwd_ref``)
+-----------------------------------------------------
+The reference is the operation in fp64 on the operands the kernel receives: bf16 ``qkv`` with q already scaled, the fp32
+bias values the kernel adds (for the LUT forms, the dense table they encode), padded keys at -inf.  The backward also
+takes the forward's bf16 ``out``, ``d_out`` and fp32 ``lse``, and defines delta_i = sum_d dO_id out_id on the given bf16
+``out`` (as the kernel and flash-attention do), so delta is part of the operation and not a source of error.  Bounds are
+absolute (``assert_within(got, ref, bound, 1.0, dtype)``; a bf16 output adds u_out |ref| there) and first order.
+
+``e_ij``   logit error, tau (|q_i| . |k_j|) + c_exp_ij + eps_b |b_ij|.  tau covers the fp32 accumulation of q.k (as for the
+           GEMM).  c_exp = 2^-19 (1 + |s_ij| + |lse_i|): __expf(x) = ex2.approx(x log2 e) is off by 2^-22 relative plus the
+           rounding of x log2 e, and x = s - m is itself rounded twice (s + b, then - m; |m| <= |lse| + log S), which is a
+           few ulps of |s| and |lse| and stays under 32 ulps of (1 + |s| + |lse|).  eps_b = 0 for the fp32 bias forms.
+           The transposed half2 tables of the backward hold fp16(b log2 e): eps_b = 2^-11 + 2^-22 (round-to-nearest to 11
+           bits, then the fp32 products), plus an absolute 2^-24 for fp16 subnormals (``EPS_B_HALF``).
+``lse``    sum_j P_ij e_ij + 2^-16 (1 + |lse_i|).  The second term is the fp32 sum of up to 750 positive exponentials (round
+           to nearest: a random walk far below 2^-16 relative), at most a dozen rescales by exp(m_old - m_new) of 2^-22
+           each, and the log.
+``out``    2^-8 (P @ |V|) + sum_j P_ij (e_ij + dlse_i) (|v_j| + |o_i|) + tau (P @ |V|), then u_out |ref|.  P.V runs on bf16 P
+           (2^-9 relative under round-to-nearest, doubled for margin, whatever the key blocking) while the denominator is
+           summed from the unrounded fp32 values, so the rounding does not cancel.  A relative error d_j of P_ij moves
+           o_i = sum_j P_ij v_j / sum_j P_ij by sum_j P_ij d_j (v_j - o_i); |v_j - o_i| <= |v_j| + |o_i|.
+``ln_stats`` per (head, row) sum and sum of squares of the 64 fp32 outputs before rounding: the ``out`` bound (without
+           u_out) carried through both sums, plus tau of the fp32 sums of |o| and o^2.
+``dV``     sum_i P_ij (2^-8 + e'_ij) |dO_i| + tau P^T |dO|, where e'_ij = e_ij + |lse_given_i - lse_i| is the error of the
+           recomputed P (the backward recomputes P from the given lse, so its actual error enters).
+``dS``     dS_ij = P_ij (dP_ij - delta_i), dP = dO V^T.  err(dS_ij) = P_ij (|dP_ij - delta_i| e'_ij + tau (|dO_i| . |v_j| +
+           sum_d |dO_id| |out_id|)): the error of P scales dP - delta, tau covers the fp32 dot products of dP and delta.
+``dbias``  sum_b dS_b over the batch for a shared table (fp32 atomics onto the initial values: + (B + 1) 2^-24 (|init| +
+           sum_b |dS_b|)); dS_b alone for per-sample tables.  Centring a row, c_ij = d_ij - mean_j d_ij, is exact in fp64;
+           the bound becomes err_ij + mean_j err_ij + S 2^-24 sum_j |d_ij| (the fp32 row sum).
+``dQ, dK`` dQ = q_scale bf16(dS) @ K and dK = bf16(dS)^T @ Q: (2^-8 |dS| + err(dS)) @ |K or Q| + tau |dS| @ |K or Q| (times
+           q_scale for dQ), then u_out |ref|.
 """
 from types import SimpleNamespace
 
@@ -282,3 +316,111 @@ def argmax_ok(z, dz, got):
     g = got.long()
     zg = z[rows, g]
     return zg >= z[rows, ref] - dz[rows, g] - dz[rows, ref]
+
+
+# ----------------------------------------------------------------------------------------------------------------------
+# attention (module docstring, "Attention")
+# ----------------------------------------------------------------------------------------------------------------------
+HD = 64                                 # head dim of every attention kernel
+C_EXP = 2.0 ** -19
+LSE_REL = 2.0 ** -16
+EPS_B_HALF = (2.0 ** -11 + 2.0 ** -22, 2.0 ** -24)       # (relative, absolute) logit error of the fp16 transposed tables
+
+
+def split_qkv(qkv, B, S, H):
+    """bf16 [B*S, 3*H*64] -> fp64 q, k, v of shape [B, H, S, 64]"""
+    t = qkv.double().view(B, S, 3, H, HD).permute(2, 0, 3, 1, 4)
+    return t[0], t[1], t[2]
+
+
+def heads_to_rows(t, B, S, H):
+    """[B, H, S, 64] -> [B*S, H*64] (the row layout of the attention output and of each third of dqkv)"""
+    return t.permute(0, 2, 1, 3).reshape(B * S, H * HD)
+
+
+def _logits(qkv, bias, key_pad, B, S, H, eps_b):
+    """scores s = q k^T + b with padded keys at -inf, and the parts of the logit error e (without c_exp, which needs lse)"""
+    q, k, v = split_qkv(qkv, B, S, H)
+    s = q @ k.transpose(-1, -2)
+    e = TAU * (q.abs() @ k.abs().transpose(-1, -2))
+    if bias is not None:
+        b = bias.double()
+        b = b if b.dim() == 4 else b[None]
+        s = s + b
+        if eps_b:
+            e = e + eps_b[0] * b.abs() + eps_b[1]
+    dead = torch.zeros(B, 1, 1, S, dtype=torch.bool, device=qkv.device)
+    if key_pad is not None:
+        dead = key_pad.bool().view(B, 1, 1, S)
+    s = s.masked_fill(dead, float("-inf"))
+    return q, k, v, s, e, dead
+
+
+def attention_ref(qkv, bias, key_pad, B, S, H, eps_b=None):
+    """fp64 attention forward and its bounds (module docstring).  bias: the values the kernel adds, fp32 (H,S,S) shared or
+    (B,H,S,S) per sample (logical columns only), or None; key_pad uint8 (B,S) or None; eps_b: EPS_B_HALF for the fp16
+    tables.  Every row needs a live key.
+
+    Returns a namespace with out / out_err [B*S, H*64], lse / dlse [B, H, S], stats / stats_err [H, B*S, 2] (the
+    ln_stats records), and p, e (P and the logit error, [B, H, S, S]) for ``attention_bwd_ref``."""
+    q, k, v, s, e, dead = _logits(qkv, bias, key_pad, B, S, H, eps_b)
+    lse = torch.logsumexp(s, -1)
+    p = (s - lse[..., None]).exp()
+    sf = torch.where(dead, torch.zeros_like(s), s)
+    e = (e + C_EXP * (1 + sf.abs() + lse.abs()[..., None])).masked_fill(dead, 0.0)
+    pe = p * e
+    dlse = pe.sum(-1) + LSE_REL * (1 + lse.abs())
+    o = p @ v
+    pv = p @ v.abs()
+    w = pe + p * dlse[..., None]                        # sum_j P_ij (e_ij + dlse_i) (|v_j| + |o_i|)
+    oerr = (2.0 ** -8 + TAU) * pv + w @ v.abs() + w.sum(-1, keepdim=True) * o.abs()
+    st = torch.stack([o.sum(-1), (o * o).sum(-1)], -1)                                        # [B, H, S, 2]
+    st_err = torch.stack([oerr.sum(-1) + TAU * o.abs().sum(-1),
+                          (2 * o.abs() * oerr + oerr * oerr).sum(-1) + TAU * (o * o).sum(-1)], -1)
+    to_rec = lambda t: t.permute(1, 0, 2, 3).reshape(H, B * S, 2)
+    return SimpleNamespace(out=heads_to_rows(o, B, S, H), out_err=heads_to_rows(oerr, B, S, H), lse=lse, dlse=dlse,
+                           stats=to_rec(st), stats_err=to_rec(st_err), p=p, e=e)
+
+
+def attention_bwd_ref(qkv, out, d_out, lse, bias, key_pad, B, S, H, q_scale, eps_b=None):
+    """fp64 attention backward on the operands of the backward call and its bounds (module docstring).  out, d_out bf16
+    [B*S, H*64]; lse fp32 [B*H*S] as given to the kernel; bias and key_pad as for ``attention_ref``.
+
+    Returns a namespace with dqkv / dqkv_err [B*S, 3*H*64] and dS, dS_err [B, H, S, S] for ``dbias_ref``."""
+    f = attention_ref(qkv, bias, key_pad, B, S, H, eps_b)
+    q, k, v = split_qkv(qkv, B, S, H)
+    do = d_out.double().view(B, S, H, HD).permute(0, 2, 1, 3)
+    o = out.double().view(B, S, H, HD).permute(0, 2, 1, 3)
+    p = f.p
+    ep = f.e + (lse.double().view(B, H, S) - f.lse).abs()[..., None]
+    dp = do @ v.transpose(-1, -2)
+    delta = (do * o).sum(-1, keepdim=True)
+    ds = p * (dp - delta)
+    ds_err = p * ((dp - delta).abs() * ep + TAU * (do.abs() @ v.abs().transpose(-1, -2) + (do.abs() * o.abs()).sum(-1, keepdim=True)))
+    dv = p.transpose(-1, -2) @ do
+    dv_err = ((2.0 ** -8 + TAU) * p + p * ep).transpose(-1, -2) @ do.abs()
+    a = 2.0 ** -8 * ds.abs() + ds_err + TAU * ds.abs()
+    dq = q_scale * (ds @ k)
+    dq_err = abs(q_scale) * (a @ k.abs())
+    dk = ds.transpose(-1, -2) @ q
+    dk_err = a.transpose(-1, -2) @ q.abs()
+    rows = lambda *ts: torch.cat([heads_to_rows(t, B, S, H) for t in ts], 1)
+    return SimpleNamespace(dqkv=rows(dq, dk, dv), dqkv_err=rows(dq_err, dk_err, dv_err), dS=ds, dS_err=ds_err, fwd=f)
+
+
+def dbias_ref(r, init, launches=1, per_sample=False):
+    """the bias gradient the backward accumulates onto ``init`` (fp32, logical columns): sum_b dS_b for a shared table
+    ((H,S,S); ``launches`` backward calls on the same operands add into it), dS_b for per-sample tables ((B,H,S,S)).
+    Returns (value, bound); the fp32 additions add (adds + 1) 2^-24 (|init| + sum |terms|)."""
+    i = init.double()
+    if per_sample:
+        d, err, mag, adds = r.dS, r.dS_err, r.dS.abs(), 1
+    else:
+        d, err, mag, adds = launches * r.dS.sum(0), launches * r.dS_err.sum(0), launches * r.dS.abs().sum(0), launches * r.dS.shape[0]
+    return i + d, err + (adds + 1) * U32 * (i.abs() + mag)
+
+
+def center_ref(d, err):
+    """row-centred bias gradient c_ij = d_ij - mean_j d_ij over the S logical columns, and its bound"""
+    S = d.shape[-1]
+    return d - d.mean(-1, keepdim=True), err + err.mean(-1, keepdim=True) + S * U32 * d.abs().sum(-1, keepdim=True)

@@ -1,6 +1,7 @@
 """CPU: the fp64 reference and per-element bounds of tests/kernel_ref.py.  A correct kernel, emulated here in fp32 (bf16
-operands, fp32 matmul, the epilogue and the LayerNorm statistics in fp32 as the kernel evaluates them), must pass the
-bounds; each of the subtle mistakes a GEMM or InfoNCE kernel can make must fail them."""
+operands, fp32 matmul, the epilogue and the LayerNorm statistics in fp32 as the kernel evaluates them; for attention the
+blocked online soft-max and the recomputing backward), must pass the bounds; each of the subtle mistakes a GEMM, InfoNCE
+or attention kernel can make must fail them."""
 import pytest
 import torch
 
@@ -165,3 +166,198 @@ def test_canary_helpers():
     out32[:3] = 0.0                            # ... and a row that should have been written must not
     with pytest.raises(AssertionError, match="not finite"):
         R.assert_canary(buf32, out32)
+
+
+# ----------------------------------------------------------------------------------------------------------------------
+# attention
+# ----------------------------------------------------------------------------------------------------------------------
+AB, AS, AH = 2, 197, 2              # S = 197: three full 64-key blocks and a partial one of 5 keys
+PAD_FROM = (195, 127)               # first padded key per sample: odd, so a pair (even live key, odd padded key) straddles
+                                    # each edge; sample 0 keeps three live keys in the last block, sample 1's padding
+                                    # covers the whole third 64-key block and the fourth
+SPLIT = 60                          # two-segment LUT: segments [0, 60) and [60, 197)
+Q_SCALE = 0.125
+LOG2E, LN2 = 1.4426950408889634, 0.69314718055994531
+
+
+@pytest.fixture(scope="module")
+def att():
+    g = torch.Generator().manual_seed(11)
+    B, S, H = AB, AS, AH
+    kp = torch.zeros(B, S, dtype=torch.uint8)
+    for b, p in enumerate(PAD_FROM):
+        kp[b, p:] = 1
+    s1, s2 = SPLIT, S - SPLIT
+    return dict(
+        qkv=(torch.randn(B * S, 3 * H * 64, generator=g) * 0.3).bfloat16(), kp=kp,
+        bias=torch.randn(H, S, S, generator=g), bias_ps=torch.randn(B, H, S, S, generator=g),
+        d_out=(torch.randn(B * S, H * 64, generator=g) * 0.5).bfloat16(), dbias0=0.01 * torch.randn(H, S, S, generator=g),
+        # two-segment LUT form: per segment a Toeplitz LUT (code difference i - j), the second segment's row codes shifted
+        # past the first segment's LUT
+        lut=torch.randn(H, (2 * s1 - 1) + (2 * s2 - 1), generator=g),
+        code_row=torch.cat([torch.arange(s1) + s1 - 1, torch.arange(s2) + s2 - 1 + 2 * s1 - 1]),
+        code_col=torch.cat([torch.arange(s1), torch.arange(s2)]))
+
+
+def lut_dense(d, mutation=None):
+    """the (H,S,S) bias the two-segment LUT form encodes, as the kernel gathers it"""
+    S = AS
+    col = d["code_col"].clone()
+    if mutation == "seg_code_col_off_by_one":       # the first key of the second segment reads the previous key's code
+        col[SPLIT] = col[SPLIT - 1]
+    i, j = torch.arange(S)[:, None], torch.arange(S)[None, :]
+    t = d["lut"][:, (d["code_row"][i] - col[j]).clamp(0, d["lut"].shape[1] - 1)]
+    if mutation == "seg_cross_not_zeroed":
+        return t
+    return torch.where((i < SPLIT) == (j < SPLIT), t, torch.zeros_like(t))
+
+
+def half_table(bias, mutation=None):
+    """the bias the transposed-table backward adds: fp16(b log2 e) ln 2, evaluated in fp32"""
+    t = (bias * LOG2E).half().float() * LN2
+    if mutation == "half2_pair_swapped":            # query rows q and q + 1 of each half2 word exchanged
+        S = t.shape[-2]
+        src = torch.arange(S) ^ 1
+        t = torch.where((src < S)[:, None], t[..., src.clamp(max=S - 1), :], torch.zeros_like(t))
+    return t
+
+
+def _f32_qkv(qkv):
+    t = qkv.float().view(AB, AS, 3, AH, 64).permute(2, 0, 3, 1, 4)
+    return t[0], t[1], t[2]
+
+
+def emulate_attention_fwd(qkv, bias, kp, mutation=None):
+    """fp32 emulation of a correct forward kernel: 64-key blocks, online soft-max with a running max, bf16 P in P.V with
+    the denominator summed from the unrounded values, lse = m + log l.  bias: (1 or B, H, S, S)."""
+    B, S, H = AB, AS, AH
+    q, k, v = _f32_qkv(qkv)
+    nb = (S + 63) // 64
+    grow = lambda t: torch.nn.functional.pad(t, (0, 0, 0, nb * 64 - S))
+    k, v = grow(k), grow(v)
+    b = torch.nn.functional.pad(bias, (0, nb * 64 - S))
+    keys = torch.arange(nb * 64)
+    kpad = torch.nn.functional.pad(kp.bool(), (0, nb * 64 - S))
+    dead = (keys >= S)[None, :] | kpad
+    if mutation == "key_S_live":                     # the key == S of the partial last block taken as live
+        dead[:, S] = False
+    if mutation == "dead_pair":                      # the odd key of a pair masked with its even partner's pad flag
+        dead = (keys >= S)[None, :] | kpad[:, keys & ~1]
+    if mutation == "bias_cols_shifted_2":            # one key block reads its bias two columns late
+        b = b.clone()
+        b[..., 64:128] = torch.nn.functional.pad(bias, (0, nb * 64 + 2 - S))[..., 66:130]
+    dead = dead.view(B, 1, 1, -1)
+    m = torch.full((B, H, S), float("-inf"))
+    l = torch.zeros(B, H, S)
+    o = torch.zeros(B, H, S, 64)
+    for kb in range(nb):
+        sl = slice(kb * 64, kb * 64 + 64)
+        s = (q @ k[..., sl, :].transpose(-1, -2) + b[..., sl]).masked_fill(dead[..., sl], float("-inf"))
+        mn = torch.maximum(m, s.amax(-1))
+        base = torch.where(mn == float("-inf"), torch.zeros_like(mn), mn)
+        corr = (m - base).exp()
+        m_prev, m = m, mn
+        p = (s - base[..., None]).exp()
+        l = l * (1.0 if mutation == "no_rescale_l" and kb == 1 else corr) + p.sum(-1)
+        o = o * (1.0 if mutation == "no_rescale_o" and kb == 1 else corr[..., None]) + p.bfloat16().float() @ v[..., sl, :]
+    lse = (m_prev if mutation == "lse_previous_max" else m) + l.log()
+    of = o / l[..., None]
+    st = torch.stack([of.sum(-1), (of * of).sum(-1)], -1).permute(1, 0, 2, 3).reshape(H, B * S, 2)
+    return R.heads_to_rows(of, B, S, H).bfloat16(), lse, st
+
+
+def emulate_attention_bwd(qkv, out, d_out, lse, bias, kp, mutation=None):
+    """fp32 emulation of a correct backward: P recomputed from the given lse, bf16 P and dS in the products, fp32 dS
+    returned for the bias gradient"""
+    B, S, H = AB, AS, AH
+    q, k, v = _f32_qkv(qkv)
+    do = d_out.float().view(B, S, H, 64).permute(0, 2, 1, 3)
+    o = out.float().view(B, S, H, 64).permute(0, 2, 1, 3)
+    L = lse.view(B, H, S)
+    dl = (do * o).sum(-1)
+    if mutation == "row_g_reads_g8":                 # rows g of each 16-row fragment read row g + 8's lse and delta
+        r = torch.arange(S)
+        src = torch.where(r % 16 < 8, (r + 8).clamp(max=S - 1), r)
+        L, dl = L[..., src], dl[..., src]
+    s = (q @ k.transpose(-1, -2) + bias).masked_fill(kp.bool().view(B, 1, 1, S), float("-inf"))
+    p = (s - L[..., None]).exp()
+    ds = p * (do @ v.transpose(-1, -2) - dl[..., None])
+    dv = p.bfloat16().float().transpose(-1, -2) @ do
+    dq = (ds.bfloat16().float() @ k) * (1.0 if mutation == "dq_without_q_scale" else Q_SCALE)
+    dk = ds.bfloat16().float().transpose(-1, -2) @ q
+    rows = lambda t: R.heads_to_rows(t, B, S, H)
+    return torch.cat([rows(dq), rows(dk), rows(dv)], 1).bfloat16(), ds
+
+
+FWD_FORMS = {"key_S_live": "dense", "dead_pair": "dense", "bias_cols_shifted_2": "dense", "no_rescale_o": "dense",
+             "no_rescale_l": "dense", "lse_previous_max": "dense", "sample_1_reads_sample_0": "per_sample",
+             "seg_cross_not_zeroed": "two_segment", "seg_code_col_off_by_one": "two_segment"}
+BWD_FORMS = {"row_g_reads_g8": "dense", "dq_without_q_scale": "dense", "half2_pair_swapped": "transposed",
+             "dbias_t_launch_lost": "transposed", "fold_swaps_query_and_key": "transposed"}
+
+
+def attention_outputs(d, form, mutation=None):
+    """{name: (got, ref, bound, dtype)} for the emulated kernel (with an optional mistake) against the references"""
+    B, S, H = AB, AS, AH
+    bias = {"dense": d["bias"], "transposed": d["bias"], "per_sample": d["bias_ps"], "two_segment": lut_dense(d)}[form]
+    seen = bias
+    if mutation == "sample_1_reads_sample_0":
+        seen = torch.stack([bias[0], bias[0]])
+    if form == "two_segment":
+        seen = lut_dense(d, mutation)
+    seen = seen if seen.dim() == 4 else seen[None]
+    out, lse, st = emulate_attention_fwd(d["qkv"], seen, d["kp"], mutation)
+    fr = R.attention_ref(d["qkv"], bias, d["kp"], B, S, H)
+    res = {"out": (out, fr.out, fr.out_err, torch.bfloat16), "lse": (lse, fr.lse, fr.dlse, torch.float32),
+           "ln_stats": (st, fr.stats, fr.stats_err, torch.float32)}
+    if form not in ("dense", "per_sample", "transposed") or mutation in FWD_FORMS:
+        return res
+    # the backward runs on the forward's outputs, as in training
+    out, lse, _ = emulate_attention_fwd(d["qkv"], bias if bias.dim() == 4 else bias[None], d["kp"])
+    eps_b = R.EPS_B_HALF if form == "transposed" else None
+    bseen = half_table(bias, mutation) if form == "transposed" else bias
+    dqkv, ds = emulate_attention_bwd(d["qkv"], out, d["d_out"], lse, bseen, d["kp"], mutation)
+    br = R.attention_bwd_ref(d["qkv"], out, d["d_out"], lse, bias, d["kp"], B, S, H, Q_SCALE, eps_b=eps_b)
+    res["dqkv"] = (dqkv, br.dqkv, br.dqkv_err, torch.bfloat16)
+    if form == "per_sample":
+        db, dbe = R.dbias_ref(br, d["dbias0"][None].expand(B, H, S, S), per_sample=True)
+        res["dbias"] = (d["dbias0"] + ds, db, dbe, torch.float32)
+    elif form == "dense":
+        db, dbe = R.dbias_ref(br, d["dbias0"])
+        res["dbias"] = (d["dbias0"] + ds.sum(0), db, dbe, torch.float32)
+    else:
+        # two launches accumulate into the transposed table, which is folded onto dbias and centred
+        launches = 1 if mutation == "dbias_t_launch_lost" else 2
+        acc = torch.zeros(H, S, S)
+        for _ in range(launches):
+            acc = acc + ds.sum(0)
+        if mutation == "fold_swaps_query_and_key":
+            acc = acc.transpose(-1, -2)
+        got = d["dbias0"] + acc
+        got = got - got.sum(-1, keepdim=True) / S
+        db, dbe = R.center_ref(*R.dbias_ref(br, d["dbias0"], launches=2))
+        res["dbias"] = (got, db, dbe, torch.float32)
+    return res
+
+
+def _ratio(got, ref, bound, dt):
+    """largest |got - ref| / bound (the fraction of the bound used; inf for a NaN)"""
+    err = (got.double() - ref.double()).abs()
+    tol = bound + (2.0 ** -8 * ref.double().abs() if dt == torch.bfloat16 else 0.0)
+    return torch.nan_to_num(torch.where(err == 0, torch.zeros_like(err), err / tol), nan=float("inf")).max().item()
+
+
+@pytest.mark.parametrize("form", ["dense", "per_sample", "two_segment", "transposed"])
+def test_attention_emulation_passes(att, form):
+    for name, (got, ref, bound, dt) in attention_outputs(att, form).items():
+        R.assert_within(got, ref, bound, 1.0, dt, what=f"{form} {name}")
+
+
+@pytest.mark.parametrize("mutation", list(FWD_FORMS) + list(BWD_FORMS))
+def test_attention_mutation_fails(att, mutation):
+    """each mistake exceeds the bound at least ten-fold on at least one output (run with -s to see the factors)"""
+    form = FWD_FORMS.get(mutation) or BWD_FORMS[mutation]
+    ratios = {name: _ratio(*v) for name, v in attention_outputs(att, form, mutation).items()}
+    name = max(ratios, key=ratios.get)
+    print(f"{mutation}: {name} exceeds its bound {ratios[name]:.3g}-fold")
+    assert ratios[name] >= 10, ratios
