@@ -324,7 +324,8 @@ int opb_geglu_bwd(const void* gl, const void* du, void* dgl, int64_t rows, int F
 
 /* LayerScale + drop-path residual (transformer_layer.py:70-88): out = x + row_scale[r] * gamma[n] * o  (o bf16; gamma /
  * row_scale may be NULL = 1) and its adjoint: d_o = bf16(row_scale * gamma * dx), dgamma = sum_r row_scale * dx * o,
- * dbias = sum_r d_o (the bias gradient of the Linear that produced o). */
+ * dbias = sum_r row_scale * gamma * dx in fp32, before the bf16 rounding of d_o (the bias gradient of the Linear that
+ * produced o; opb_colsum_bf16 instead sums the rounded values it is given). */
 int opb_scale_resid_fwd(const float* x, const void* o, const float* gamma, const float* row_scale, float* out,
                         int64_t rows, int n, void* stream);
 int opb_scale_resid_bwd(const float* dx, const void* o, const float* gamma, const float* row_scale, void* d_o, float* ws,

@@ -388,7 +388,8 @@ scale_resid_bwd_kernel(const float* __restrict__ dx, const __nv_bfloat16* __rest
           dg[k].x += d.x * ov.x; dg[k].y += d.y * ov.y; dg[k].z += d.z * ov.z; dg[k].w += d.w * ov.w;
         }
         d.x *= gm[k].x; d.y *= gm[k].y; d.z *= gm[k].z; d.w *= gm[k].w;
-        // the bias gradient sums the bf16-rounded values the dW GEMM also consumes
+        // d_o is rounded to bf16 for the dW GEMM; the bias gradient sums the unrounded fp32 d (colsum, which serves
+        // passes that only have d_o, sums the rounded values instead)
         uint2 pk;
         pk.x = pack_bf16x2(d.x, d.y);
         pk.y = pack_bf16x2(d.z, d.w);

@@ -1,6 +1,7 @@
-"""fp64 references of the GEMM epilogues (csrc/gemm_wgmma.cu), of the contrastive-head reductions (csrc/infonce.cu) and of
-the attention forward and backward (csrc/attention.cu, csrc/attention_bwd.cu), with an error bound for every output
-element, and NaN-canary output buffers.
+"""fp64 references of the GEMM epilogues (csrc/gemm_wgmma.cu), of the contrastive-head reductions (csrc/infonce.cu), of
+the attention forward and backward (csrc/attention.cu, csrc/attention_bwd.cu) and of the row kernels (csrc/layernorm.cu,
+csrc/backward.cu, csrc/pack.cu, csrc/gather.cu), with an error bound for every output element, and NaN-canary output
+buffers.
 
 Plain PyTorch on whatever device the inputs live on; nothing here calls the extension.
 
@@ -58,6 +59,52 @@ absolute (``assert_within(got, ref, bound, 1.0, dtype)``; a bf16 output adds u_o
            the bound becomes err_ij + mean_j err_ij + S 2^-24 sum_j |d_ij| (the fp32 row sum).
 ``dQ, dK`` dQ = q_scale bf16(dS) @ K and dK = bf16(dS)^T @ Q: (2^-8 |dS| + err(dS)) @ |K or Q| + tau |dS| @ |K or Q| (times
            q_scale for dQ), then u_out |ref|.
+
+Row kernels (``layernorm_ref``, ``layernorm_bwd_ref`` and the functions after them)
+----------------------------------------------------------------------------------
+Bounds are absolute (``assert_within(got, ref, bound, 1.0, dtype)``), first order, u = 2^-24.  Every fp32 reduction in these
+kernels is at most 256 additions deep (a row: <= 24 per thread, 5 shuffle levels, <= 8 warps; a column: <= 48 rows per CTA
+at 12608 rows, <= 10 + 32 steps in ``partial_reduce_kernel``), so tau = 2^-16 >= 256 u bounds its worst case, in any order.
+
+``fast_erf``  Abramowitz-Stegun 7.1.26 (|error| <= 1.5e-7) evaluated in fp32 with rcp.approx (1 ulp) and ex2.approx (2^-22
+           relative).  Near x = 0, 1 - p e cancels: eight roundings of values near 1 add <= 5e-7, rcp moves p e by
+           |t p'(t)| e 2^-23 <= 3e-7, ex2 by 2^-22 p e <= 2.4e-7: ERF_ABS = 2^-19 (1.9e-6) covers the sum, 1.2e-6.
+           gelu_erf(y) = 0.5 y (1 + erf(y / sqrt 2)) is then off by |y| GELU_REL, GELU_REL = ERF_ABS / 2 + 4 u.
+           gelu_grad(z) = Phi(z) + z phi(z) with phi from __expf (2 + 1.173 |x| ulps): GELU_GRAD_ABS = ERF_ABS / 2 + 2^-21
+           (the z phi(z) (2 + 0.59 z^2) 2^-23 <= 2^-23 term and the roundings).  tests/test_kernel_ref.py evaluates an fp32
+           port with every approximation perturbed by its limit and checks all three constants.  An error dz of the
+           argument moves gelu by <= 1.13 dz and gelu' by <= 0.8 dz (max |gelu''| = 2 phi(0)).
+``layernorm`` (two-pass statistics, one warp per row)  With a1 = mean |x|:  dmu = (tau + u) a1;  the centred sum of squares
+           about the rounded mean is var + dmu^2 exactly, so dvar = (tau + 3u) var + dmu^2;  rel(rstd) = dvar / (2 (var +
+           eps)) + 2^-22 (rsqrtf; every rel here uses the form of ``ln_stats_ref`` that stays exact for large dvar);
+           xhat: rstd (dmu + u |x - mu|) + |xhat| (rel + u);  affine: |g| dxhat + 2u (|xhat g| + |b|);  gelu: 1.13 dy +
+           |y| GELU_REL;  fp32 ``accumulate``: + u (|prev| + |y|);  then u_out |ref|.  ``raw`` writes bf16(x) (bit-exact)
+           and mu / rstd with the bounds dmu and rel.
+``layernorm_bwd``  dx = rstd (dy g - m1 - xhat m2), m1 = mean(dy g), m2 = mean(dy g xhat).  The plain path reduces in one
+           pass about K = x[row][0]: ms = mean(x - K), var = mean((x - K)^2) - ms^2.  With A = mean |x - K| and
+           Q = mean (x - K)^2 = var + ms^2:  dms = (tau + u) A;  dvar = (tau + 2u) Q + 2 A dms + dms^2 (the Q / var factor
+           is the cancellation, small while K is near the mean, large for an outlier in column 0 or |mean| / std ~ 10^3);
+           m2 = rstd mean(dy g (x - K - ms)) is off by rstd ((tau + 2u) mean |dy g| |x - K| + |ms| dm1 + |m1| dms +
+           2u |ms m1|) + |m2| (rel + u).  The gelu path runs two-pass statistics as the forward and first multiplies dy by
+           gelu'(z), z = xhat g + b (dz = |g| dxhat + u |z|, d gelu' = 0.8 dz + GELU_GRAD_ABS).  Both paths then give
+           dx: rstd (d(dy g) + dm1 + |xhat| dm2 + |m2| dxhat + 2u (|dy g| + |m1| + |xhat m2|)) + |dx| (rel + u).
+           dgamma = sum_rows dy' xhat and dbeta = sum_rows dy' (dy' = dy, or dy gelu'(z)): sum of the terms' errors plus
+           (tau + u) sum |terms|.
+``geglu``  u = gelu(g) l: |l| |g| GELU_REL + 2u |u|.  Backward: dg = du l gelu'(g): |du l| GELU_GRAD_ABS + 3u |dg|;
+           dl = du gelu(g): |du g| GELU_REL + u |dl|.  bf16 outputs add u_out |ref|.
+``scale_resid``  forward out = x + rs gamma o: 2u (|rs gamma o| + |out|).  Backward d = rs gamma dx (2u |d|), d_o = bf16(d);
+           dgamma = sum_rows rs dx o and dbias = sum_rows d, both with (tau + 2u) sum |terms|.  dbias sums the fp32 values d,
+           not the rounded d_o (the fp32 value is the better estimate of the true gradient; ``colsum`` serves the passes
+           that only have d_o and sums exactly those bf16 values).
+``colsum``  sum of the given bf16 values: tau sum |y|.
+``ln_fold``  Wg = bf16(fp32(W g)) is bit-exact; colsum = sum_k Wg (the rounded values): tau sum |Wg|; bias' = W beta + b:
+           (tau + u) sum |W| |beta| + u (|bias'| + |b|).
+``l2_normalize_bwd``  dx = dy / |x| - x (x . dy) / |x|^3.  The fp32 norm is off by rel_n = (tau + 2u) / 2 + u relative,
+           1 / |x| by rel_n + u; k = (x . dy) / |x|^3 by (tau + u) sum |x dy| / |x|^3 + |k| (3 rel_n + 4u); dx: |dy| / |x|
+           (rel_n + 2u) + |x| dk + u (|x k| + |dx|).
+scatter-adds  (fp32 atomics, ``batch_sum``): onto init, count contributions in any order: (count + 1) u (|init| + sum |g|)
+           per destination element.  ``window_scatter`` sums <= kw bf16 terms in a fixed order: kw u sum |terms|, then
+           u_out |ref|.
 """
 from types import SimpleNamespace
 
@@ -85,8 +132,12 @@ def ln_stats_ref(records, parts, M, dim, eps):
       |d E2|   <= P u E[x^2]                                 (sum of non-negative records, then the division)
       |d mu^2| <= 2 |mu| |d mu| + u mu^2
       |d var|  <= (P + 2) u (E[x^2] + 2 |mu| a1)             (mu^2 <= E[x^2], var <= E[x^2])
-    so rstd is off by at most |d var| / (2 (var + eps)) relative, plus 2^-22 for rsqrtf (2 ulp).  The E[x^2] / var factor is
-    the cancellation of E[x^2] - mu^2 for rows whose mean is large against their spread."""
+    so rstd is off by at most |d var| / (2 (var + eps)) relative to first order, plus 2^-22 for rsqrtf (2 ulp).  The
+    E[x^2] / var factor is the cancellation of E[x^2] - mu^2 for rows whose mean is large against their spread.  Where
+    |d var| is not small against var + eps (|mean| / std ~ 10^3 over many records), the first-order form no longer holds:
+    the computed variance can fall to 0 and rstd rise to 1 / sqrt(eps).  rsqrt is decreasing and convex, so rstd rises by
+    at most rsqrt(max(var - |d var|, 0) + eps) / rstd - 1 (exact) and falls by at most |d var| / (2 (var + eps)) (the
+    first-order value bounds the fall); ``rel`` is the larger of the two."""
     r = records.reshape(parts, M, 2).double()
     s1, s2 = r[..., 0].sum(0), r[..., 1].sum(0)
     mu, ex2 = s1 / dim, s2 / dim
@@ -94,7 +145,8 @@ def ln_stats_ref(records, parts, M, dim, eps):
     rstd = (var + eps).rsqrt()
     a1 = r[..., 0].abs().sum(0) / dim
     dmu = parts * U32 * a1 + U32 * mu.abs()
-    rel = (parts + 2) * U32 * (ex2 + 2 * mu.abs() * a1) / (2 * (var + eps)) + 2.0 ** -22
+    dvar = (parts + 2) * U32 * (ex2 + 2 * mu.abs() * a1)
+    rel = _rstd(var, dvar, eps)[1]
     return mu, rstd, dmu, rel
 
 
@@ -424,3 +476,244 @@ def center_ref(d, err):
     """row-centred bias gradient c_ij = d_ij - mean_j d_ij over the S logical columns, and its bound"""
     S = d.shape[-1]
     return d - d.mean(-1, keepdim=True), err + err.mean(-1, keepdim=True) + S * U32 * d.abs().sum(-1, keepdim=True)
+
+
+# ----------------------------------------------------------------------------------------------------------------------
+# row kernels (module docstring, "Row kernels")
+# ----------------------------------------------------------------------------------------------------------------------
+ERF_ABS = 2.0 ** -19
+GELU_REL = ERF_ABS / 2 + 4 * U32
+GELU_GRAD_ABS = ERF_ABS / 2 + 2.0 ** -21
+GELU_CURV = 0.8                 # max |gelu''(z)| = 2 phi(0) = 0.798
+RSQRT_REL = 2.0 ** -22
+
+
+def gelu_grad(z):
+    """exact d/dz gelu(z) = Phi(z) + z phi(z)"""
+    return 0.5 * (1 + torch.special.erf(z / 2 ** 0.5)) + z * torch.exp(-0.5 * z * z) / (2 * np.pi) ** 0.5
+
+
+def _vec(v, n, fill, like):
+    return v.double() if v is not None else torch.full((n,), fill, dtype=torch.float64, device=like.device)
+
+
+def _rstd(var, dvar, eps):
+    """rstd and its relative bound, exact in dvar (``ln_stats_ref``)"""
+    rstd = (var + eps).rsqrt()
+    rise = (var - dvar).clamp_min(0.0).add(eps).rsqrt() / rstd - 1
+    return rstd, torch.maximum(rise, dvar / (2 * (var + eps))) + RSQRT_REL
+
+
+def layernorm_ref(x, gamma, beta, eps, *, gelu=False, prev=None):
+    """fp64 LayerNorm (``opb_layernorm``) of the logical rows x [rows, dim] (fp32 or bf16 as given to the kernel), in input
+    row order and column order (``ln_layout`` maps them to the output), and its bound.  prev: the fp32 values an
+    ``accumulate`` call adds onto (already in input row order).  Returns a namespace with y, err [rows, dim], mu, rstd,
+    dmu, rel [rows] (the ``raw`` statistics and their bounds)."""
+    X = x.double()
+    n = X.shape[1]
+    g, b = _vec(gamma, n, 1.0, X), _vec(beta, n, 0.0, X)
+    mu = X.mean(1, keepdim=True)
+    xc = X - mu
+    var = (xc * xc).mean(1, keepdim=True)
+    dmu = (TAU + U32) * X.abs().mean(1, keepdim=True)
+    rstd, rel = _rstd(var, (TAU + 3 * U32) * var + dmu * dmu, eps)
+    xh = xc * rstd
+    dxh = rstd * (dmu + U32 * xc.abs()) + xh.abs() * (rel + U32)
+    y = xh * g + b
+    err = g.abs() * dxh + 2 * U32 * ((xh * g).abs() + b.abs())
+    if gelu:
+        err = GELU_SLOPE * err + GELU_REL * y.abs()
+        y = _gelu(y)
+    if prev is not None:
+        p = prev.double()
+        err = err + U32 * (p.abs() + (y + p).abs())
+        y = y + p
+    return SimpleNamespace(y=y, err=err, mu=mu[:, 0], rstd=rstd[:, 0], dmu=dmu[:, 0], rel=rel[:, 0])
+
+
+def ln_layout(rows, dim, *, merge_grid_w=0, row_period=0, row_valid=0, out_period=0, out_row_shift=0, group_in=0,
+              group_out=0):
+    """where ``opb_layernorm`` stores input row r, column c: (out_row [rows], col [rows, dim], written [rows])."""
+    r = torch.arange(rows)
+    c = torch.arange(dim)
+    orow, col0, written = r, torch.zeros(rows, dtype=torch.long), torch.ones(rows, dtype=torch.bool)
+    if merge_grid_w:
+        w = merge_grid_w
+        xx, yy, bb = r % w, (r // w) % w, r // (w * w)
+        orow = (bb * (w // 2) + yy // 2) * (w // 2) + xx // 2
+        col0 = ((yy % 2) * 2 + xx % 2) * dim
+    if row_period:
+        orow = (r // row_period) * out_period + r % row_period + out_row_shift
+        written = (r % row_period) < row_valid
+    oc = (c // group_in) * group_out + c % group_in if group_in else c
+    return orow, col0[:, None] + oc[None, :], written
+
+
+def layernorm_bwd_ref(x, dy, gamma, beta, eps, *, gelu=False, old=None):
+    """fp64 adjoint of ``layernorm_ref`` (``opb_layernorm_bwd``): x, dy [rows, dim] logical rows as the kernel reads them
+    (dy already gathered through the merge map), old: the fp32 dx an ``accumulate`` call adds onto.  Returns a namespace
+    with dx, dx_err [rows, dim], dgamma, dgamma_err, dbeta, dbeta_err [dim]."""
+    X, G = x.double(), dy.double()
+    n = X.shape[1]
+    g, b = _vec(gamma, n, 1.0, X), _vec(beta, n, 0.0, X)
+    mu = X.mean(1, keepdim=True)
+    xc = X - mu
+    var = (xc * xc).mean(1, keepdim=True)
+    rstd = (var + eps).rsqrt()
+    xh = xc * rstd
+    mean = lambda t: t.mean(1, keepdim=True)
+    if gelu:
+        dmu = (TAU + U32) * mean(X.abs())
+        _, rel = _rstd(var, (TAU + 3 * U32) * var + dmu * dmu, eps)
+        dxh = rstd * (dmu + U32 * xc.abs()) + xh.abs() * (rel + U32)
+        z = xh * g + b
+        dz = g.abs() * dxh + U32 * z.abs()
+        gg = gelu_grad(z)
+        Gp = G * gg
+        dGp = G.abs() * (GELU_CURV * dz + GELU_GRAD_ABS) + U32 * Gp.abs()
+        dyg = Gp * g
+        ddyg = g.abs() * dGp + U32 * dyg.abs()
+        m1, m2 = mean(dyg), mean(dyg * xh)
+        dm1 = TAU * mean(dyg.abs()) + mean(ddyg)
+        dm2 = TAU * mean((dyg * xh).abs()) + mean(ddyg * xh.abs() + dyg.abs() * dxh)
+    else:
+        xs = X - X[:, :1]
+        A, Q = mean(xs.abs()), mean(xs * xs)
+        ms = mean(xs)
+        dms = (TAU + U32) * A
+        _, rel = _rstd(var, (TAU + 2 * U32) * Q + 2 * A * dms + dms * dms, eps)
+        dxh = rstd * (dms + U32 * (xs.abs() + xc.abs())) + xh.abs() * (rel + U32)
+        Gp, dGp = G, torch.zeros_like(G)
+        dyg = G * g
+        ddyg = U32 * dyg.abs()
+        m1, m2 = mean(dyg), mean(dyg * xh)
+        dm1 = (TAU + U32) * mean(dyg.abs())
+        dm2 = rstd * ((TAU + 2 * U32) * mean(dyg.abs() * xs.abs()) + ms.abs() * dm1 + m1.abs() * dms
+                      + 2 * U32 * (ms * m1).abs()) + m2.abs() * (rel + U32)
+    dx = rstd * (dyg - m1 - xh * m2)
+    dt = ddyg + dm1 + xh.abs() * dm2 + m2.abs() * dxh + 2 * U32 * (dyg.abs() + m1.abs() + (xh * m2).abs())
+    err = rstd * dt + dx.abs() * (rel + U32)
+    if old is not None:
+        o = old.double()
+        err = err + U32 * (o.abs() + (dx + o).abs())
+        dx = dx + o
+    return SimpleNamespace(dx=dx, dx_err=err,
+                           dgamma=(Gp * xh).sum(0), dgamma_err=(Gp.abs() * dxh + dGp * xh.abs()).sum(0) + (TAU + U32) * (Gp * xh).abs().sum(0),
+                           dbeta=Gp.sum(0), dbeta_err=dGp.sum(0) + (TAU + U32) * Gp.abs().sum(0))
+
+
+def merge_rows(rows, dim, w):
+    """(source row, column offset) of dy row r of ``layernorm_bwd(dy_merge_w=w)``: the forward's pixel-merge map"""
+    orow, col, _ = ln_layout(rows, dim, merge_grid_w=w)
+    return orow, col[:, 0]
+
+
+def geglu_ref(gl):
+    """u = gelu(g) l of bf16 [rows, 2F] = [g | l] -> (u, bound)"""
+    F = gl.shape[1] // 2
+    g, l = gl.double()[:, :F], gl.double()[:, F:]
+    u = _gelu(g) * l
+    return u, l.abs() * g.abs() * GELU_REL + 2 * U32 * u.abs()
+
+
+def geglu_bwd_ref(gl, du):
+    """(d[g | l], bound) of u = gelu(g) l for the bf16 upstream gradient du [rows, F]"""
+    F = gl.shape[1] // 2
+    g, l, d = gl.double()[:, :F], gl.double()[:, F:], du.double()
+    dg, dl = d * l * gelu_grad(g), d * _gelu(g)
+    return (torch.cat([dg, dl], 1),
+            torch.cat([(d * l).abs() * GELU_GRAD_ABS + 3 * U32 * dg.abs(), (d * g).abs() * GELU_REL + U32 * dl.abs()], 1))
+
+
+def scale_resid_ref(x, o, gamma, row_scale):
+    """out = x + row_scale gamma o -> (out, bound)"""
+    n = x.shape[1]
+    t = _rs(row_scale, x) * _vec(gamma, n, 1.0, x) * o.double()
+    out = x.double() + t
+    return out, 2 * U32 * (t.abs() + out.abs())
+
+
+def _rs(row_scale, like):
+    return row_scale.double()[:, None] if row_scale is not None else 1.0
+
+
+def scale_resid_rows(rows, in_period=0, in_valid=0, in_shift=0):
+    """dx row read for output row r of ``scale_resid_bwd`` (the gather behind the CLS slot)"""
+    r = torch.arange(rows)
+    return (r // in_valid) * in_period + in_shift + r % in_valid if in_valid else r
+
+
+def scale_resid_bwd_ref(dx_rows, o, gamma, row_scale):
+    """dx_rows: the dx rows the kernel reads for each output row (``scale_resid_rows``).  Returns a namespace with d_o, d_o_err
+    [rows, n], dgamma, dgamma_err, dbias, dbias_err [n] (dbias sums the fp32 values, module docstring)"""
+    n = dx_rows.shape[1]
+    rd = _rs(row_scale, dx_rows) * dx_rows.double()
+    d = rd * _vec(gamma, n, 1.0, dx_rows)
+    tg = rd * o.double() if o is not None else torch.zeros_like(rd)
+    return SimpleNamespace(d_o=d, d_o_err=2 * U32 * d.abs(), dgamma=tg.sum(0), dgamma_err=(TAU + 2 * U32) * tg.abs().sum(0),
+                           dbias=d.sum(0), dbias_err=(TAU + 2 * U32) * d.abs().sum(0))
+
+
+def colsum_ref(y):
+    Y = y.double()
+    return Y.sum(0), TAU * Y.abs().sum(0)
+
+
+def ln_fold_ref(W, g, beta, bias, interleave=0):
+    """``opb_ln_fold`` -> namespace rows (destination row of weight row n), wg (bf16 [N, K], bit-exact), colsum, colsum_err,
+    bias, bias_err [N] in weight row order"""
+    N, K = W.shape
+    gf = g.float() if g is not None else torch.ones(K, dtype=torch.float32, device=W.device)
+    wg = (W.float() * gf).bfloat16()
+    n = torch.arange(N, device=W.device)
+    rows = n if interleave == 0 else (n // 128) * 256 + n % 128 + (128 if interleave == 2 else 0)
+    Wd = W.double()
+    bt = beta.double() if beta is not None else torch.zeros(K, dtype=torch.float64, device=W.device)
+    b0 = bias.double() if bias is not None else torch.zeros(N, dtype=torch.float64, device=W.device)
+    bs = Wd @ bt + b0
+    return SimpleNamespace(rows=rows, wg=wg, colsum=wg.double().sum(1), colsum_err=TAU * wg.double().abs().sum(1), bias=bs,
+                           bias_err=(TAU + U32) * (Wd.abs() @ bt.abs()) + U32 * (bs.abs() + b0.abs()))
+
+
+def l2_normalize_bwd_ref(x, dy):
+    """fp64 adjoint of y = x / |x| (``opb_l2_normalize_bwd``) on rows of fp32 x, dy -> (dx, bound)"""
+    X, G = x.double(), dy.double()
+    nrm = X.norm(dim=1, keepdim=True)
+    dot = (X * G).sum(1, keepdim=True)
+    k = dot / nrm ** 3
+    dx = G / nrm - X * k
+    rel_n = (TAU + 2 * U32) / 2 + U32
+    dk = (TAU + U32) * (X * G).abs().sum(1, keepdim=True) / nrm ** 3 + k.abs() * (3 * rel_n + 4 * U32)
+    return dx, G.abs() / nrm * (rel_n + 2 * U32) + X.abs() * dk + U32 * ((X * k).abs() + dx.abs())
+
+
+def scatter_ref(init, dest, src):
+    """fp64 result of fp32-atomic scatter-adds: out = init; out[dest[i]] += src[i] (rows of src [m, ...] onto rows of init
+    [n, ...]; dest [m] long, entries < 0 skipped) -> (out, bound), bound (count + 1) u (|init| + sum |src|)"""
+    I = init.double()
+    keep = dest >= 0
+    d, s = dest[keep], src.double()[keep]
+    out, mag = I.clone(), I.abs().clone()
+    cnt = torch.zeros(I.shape[0], dtype=torch.float64, device=I.device)
+    out.index_add_(0, d, s)
+    mag.index_add_(0, d, s.abs())
+    cnt.index_add_(0, d, torch.ones(d.shape[0], dtype=torch.float64, device=I.device))
+    cnt = cnt.view(-1, *([1] * (I.dim() - 1)))
+    return out, (cnt + 1) * U32 * mag
+
+
+def window_scatter_ref(dwin, B, t_in, t_out, stride, kw, pad):
+    """fp64 col2im of ``opb_window_scatter``: bf16 [groups, B*t_out, kw*cg] -> ([B*t_in, groups*cg], bound)"""
+    groups, _, kc = dwin.shape
+    cg = kc // kw
+    D = dwin.double().view(groups, B, t_out, kw, cg)
+    out = torch.zeros(B, t_in, groups, cg, dtype=torch.float64, device=dwin.device)
+    mag = torch.zeros_like(out)
+    for t in range(t_out):
+        for j in range(kw):
+            s = t * stride + j - pad
+            if 0 <= s < t_in:
+                v = D[:, :, t, j].permute(1, 0, 2)
+                out[:, s] += v
+                mag[:, s] += v.abs()
+    return out.reshape(B * t_in, groups * cg), kw * U32 * mag.reshape(B * t_in, groups * cg)

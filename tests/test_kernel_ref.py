@@ -361,3 +361,297 @@ def test_attention_mutation_fails(att, mutation):
     name = max(ratios, key=ratios.get)
     print(f"{mutation}: {name} exceeds its bound {ratios[name]:.3g}-fold")
     assert ratios[name] >= 10, ratios
+
+
+# ----------------------------------------------------------------------------------------------------------------------
+# row kernels
+# ----------------------------------------------------------------------------------------------------------------------
+def _f32(t):
+    return t.float().double()
+
+
+def _c(v):
+    return float(torch.tensor(v, dtype=torch.float32))
+
+
+def fast_erf(x, d_rcp=0.0, d_ex2=0.0):
+    """fp32 port of common.cuh fast_erf (fp64 arithmetic rounded to fp32 after each operation, an fma rounded once);
+    d_rcp / d_ex2: relative errors of rcp.approx / ex2.approx"""
+    x = x.double()
+    ax = x.abs()
+    t = _f32(_f32(1.0 / _f32(_c(0.3275911) * ax + 1.0)) * (1 + d_rcp))
+    p = _f32(_c(1.061405429) * t + _c(-1.453152027))
+    for c in (1.421413741, -0.284496736, 0.254829592):
+        p = _f32(p * t + _c(c))
+    p = _f32(p * t)
+    e = _f32(_f32(torch.exp2(_f32(_f32(_c(-1.4426950408889634) * ax) * ax))) * (1 + d_ex2))
+    return _f32(1.0 - p * e).copysign(x)
+
+
+def gelu_erf(x, **k):
+    x = x.double()
+    return _f32(_f32(0.5 * x) * _f32(1.0 + fast_erf(_f32(x * _c(0.70710678118654752440)), **k)))
+
+
+def gelu_grad(z, d_exp=0, **k):
+    """d_exp = +-1: __expf off by its documented limit, 2 + floor(1.173 |x|) ulps"""
+    z = z.double()
+    cdf = _f32(0.5 * _f32(1.0 + fast_erf(_f32(z * _c(0.70710678118654752)), **k)))
+    arg = _f32(_f32(-0.5 * z) * z)
+    e = _f32(_f32(torch.exp(arg)) * (1 + d_exp * (2 + torch.floor(1.173 * arg.abs())) * 2.0 ** -23))
+    return _f32(cdf + z * _f32(_c(0.3989422804014327) * e))
+
+
+def test_gelu_constants():
+    """the erf / gelu / gelu' allowances of kernel_ref hold for the fp32 port with every approximation at its limit"""
+    z = _f32(torch.linspace(-10, 10, 200001, dtype=torch.float64))
+    phi = torch.exp(-0.5 * z * z) / (2 * torch.pi) ** 0.5
+    Phi = 0.5 * (1 + torch.special.erf(z / 2 ** 0.5))
+    worst = [0.0, 0.0, 0.0]
+    for dr in (-2.0 ** -23, 0.0, 2.0 ** -23):
+        for de in (-2.0 ** -22, 0.0, 2.0 ** -22):
+            worst[0] = max(worst[0], (fast_erf(z, d_rcp=dr, d_ex2=de) - torch.special.erf(z)).abs().max().item())
+            worst[1] = max(worst[1], ((gelu_erf(z, d_rcp=dr, d_ex2=de) - z * Phi).abs() / z.abs().clamp_min(1e-30)).max().item())
+            for dx in (-1, 1):
+                worst[2] = max(worst[2], (gelu_grad(z, d_exp=dx, d_rcp=dr, d_ex2=de) - (Phi + z * phi)).abs().max().item())
+    print(f"erf {worst[0]:.3g} of {R.ERF_ABS:.3g}, gelu / |x| {worst[1]:.3g} of {R.GELU_REL:.3g}, "
+          f"gelu' {worst[2]:.3g} of {R.GELU_GRAD_ABS:.3g}")
+    assert worst[0] <= R.ERF_ABS and worst[1] <= R.GELU_REL and worst[2] <= R.GELU_GRAD_ABS
+
+
+LN_ROWS, LN_DIM = 300, 256          # 300 CTAs of one row each: a parts % 128 tail of 44 records
+
+
+def _ln_rows(g, rows, dim):
+    """N(0, 1) rows, then stress rows: |mean| / std ~ 10^3, an outlier in column 0, constant rows and var << eps"""
+    x = torch.randn(rows, dim, generator=g) * (1 + 0.3 * torch.rand(rows, 1, generator=g))
+    x[-8:-4] = 1000.0 + torch.randn(4, dim, generator=g)
+    x[-4, 0] += 40.0
+    x[-3] = 0.75
+    x[-2] = 0.3 + 1e-4 * torch.randn(dim, generator=g)
+    return x
+
+
+@pytest.fixture(scope="module")
+def rowk():
+    g = torch.Generator().manual_seed(21)
+    x = _ln_rows(g, LN_ROWS, LN_DIM)
+    d = dict(x=x, dy=torch.randn(LN_ROWS, LN_DIM, generator=g), gamma=1 + 0.3 * torch.randn(LN_DIM, generator=g),
+             beta=0.3 * torch.randn(LN_DIM, generator=g))
+    # gelu inputs up to |z| = 8: a wide gamma
+    d["gamma_gelu"] = 3 * torch.randn(LN_DIM, generator=g)
+    return d
+
+
+def _partials(terms, grid):
+    """column sums of terms [rows, n] as the kernel forms them: row r in CTA r % grid (fp32, in row order), then
+    partial_reduce_kernel: 32 lanes each over records p = lane (mod 32), lanes summed in order"""
+    rows = terms.shape[0]
+    part = torch.zeros(grid, terms.shape[1])
+    for r in range(rows):
+        part[r % grid] += terms[r]
+    lanes = torch.zeros(32, terms.shape[1])
+    for p in range(grid):
+        lanes[p % 32] += part[p]
+    tot = torch.zeros(terms.shape[1])
+    for k in range(32):
+        tot += lanes[k]
+    return tot, part
+
+
+def emulate_ln_bwd(d, gelu=False, mutation=None):
+    """fp32 layernorm_bwd: the plain path reduces once about K = x[row][0]; the gelu path runs two-pass statistics"""
+    X, G = d["x"].float(), d["dy"].float()
+    g = d["gamma_gelu"] if gelu else d["gamma"]
+    n = X.shape[1]
+    if gelu:
+        mean = X.sum(1, keepdim=True) / n
+        xc = X - mean
+        rstd = torch.rsqrt((xc * xc).sum(1, keepdim=True) / n + 1e-5)
+        xh = xc * rstd
+        Gp = (G.double() * gelu_grad(xh.double() * g.double() + d["beta"].double())).float()
+        gy = Gp * g
+        m1, m2 = gy.sum(1, keepdim=True) / n, (gy * xh).sum(1, keepdim=True) / n
+    else:
+        Gp = G
+        K = torch.zeros_like(X[:, :1]) if mutation == "unshifted_var" else X[:, :1]
+        xs = X - K
+        ms = xs.sum(1, keepdim=True) / n
+        rstd = torch.rsqrt(((xs * xs).sum(1, keepdim=True) / n - ms * ms).clamp_min(0) + 1e-5)
+        if mutation == "neighbour_row_stats":             # every row reads the statistics of the row after it
+            mean = torch.roll(K + ms, -1, 0)
+            rstd = torch.roll(rstd, -1, 0)
+            xs, ms = X - mean, torch.zeros_like(ms)
+        gy = G * g
+        m1 = gy.sum(1, keepdim=True) / n
+        m2 = rstd * ((gy * xs).sum(1, keepdim=True) - ms * gy.sum(1, keepdim=True)) / n
+        xh = (xs - ms) * rstd
+        if mutation == "gamma_after_sums":                 # row sums of dy, then times gamma
+            m1 = g * G.sum(1, keepdim=True) / n
+            m2 = g * rstd * ((G * xs).sum(1, keepdim=True) - ms * G.sum(1, keepdim=True)) / n
+    if mutation == "drop_xhat_term":
+        m2 = torch.zeros_like(m2)
+    dx = rstd * (gy - m1 - xh * m2)
+    grid = min(X.shape[0], 132 * 8)
+    dgamma, part = _partials(Gp * xh, grid)
+    dbeta, partb = _partials(Gp, grid)
+    if mutation == "last_partial_dropped":              # the reduction's tail loop stops one record early
+        dgamma, dbeta = dgamma - part[-1], dbeta - partb[-1]
+    return dx, dgamma, dbeta
+
+
+def ln_bwd_outputs(d, gelu=False, mutation=None):
+    dx, dg, db = emulate_ln_bwd(d, gelu, mutation)
+    r = R.layernorm_bwd_ref(d["x"], d["dy"], d["gamma_gelu"] if gelu else d["gamma"], d["beta"], 1e-5, gelu=gelu)
+    return {"dx": (dx.bfloat16(), r.dx, r.dx_err, torch.bfloat16), "dx_f32": (dx, r.dx, r.dx_err, torch.float32),
+            "dgamma": (dg, r.dgamma, r.dgamma_err, torch.float32), "dbeta": (db, r.dbeta, r.dbeta_err, torch.float32)}
+
+
+MERGE_W = 8                        # two images of an 8 x 8 grid, merged 2 x 2
+
+
+def emulate_ln_fwd(d, mutation=None):
+    """fp32 layernorm forward (two-pass statistics, fast_erf GELU) with the pixel-merge scatter, output [rows / 4, 4 dim]"""
+    X = d["x"][:2 * MERGE_W * MERGE_W].float()
+    n = X.shape[1]
+    mean = X.sum(1, keepdim=True) / n
+    xc = X - mean
+    rstd = torch.rsqrt((xc * xc).sum(1, keepdim=True) / n + 1e-5)
+    y = (xc * rstd * d["gamma_gelu"] + d["beta"]).double()
+    y = gelu_erf(y).float()
+    rows = torch.arange(X.shape[0])
+    if mutation == "merge_xy_swapped":
+        w = MERGE_W
+        rows = (rows // (w * w)) * w * w + (rows % w) * w + (rows // w) % w
+    orow, col, _ = R.ln_layout(X.shape[0], n, merge_grid_w=MERGE_W)
+    out = torch.zeros(X.shape[0] // 4, 4 * n)
+    out[orow[rows][:, None], col[rows]] = y
+    return out
+
+
+def ln_fwd_outputs(d, mutation=None):
+    X = d["x"][:2 * MERGE_W * MERGE_W]
+    r = R.layernorm_ref(X, d["gamma_gelu"], d["beta"], 1e-5, gelu=True)
+    orow, col, _ = R.ln_layout(X.shape[0], X.shape[1], merge_grid_w=MERGE_W)
+    ref = torch.zeros(X.shape[0] // 4, 4 * X.shape[1], dtype=torch.float64)
+    err = torch.zeros_like(ref)
+    ref[orow[:, None], col] = r.y
+    err[orow[:, None], col] = r.err
+    got = emulate_ln_fwd(d, mutation)
+    return {"y": (got.bfloat16(), ref, err, torch.bfloat16), "y_f32": (got, ref, err, torch.float32)}
+
+
+SR_B, SR_S = 3, 197                 # image adapter: 196 token rows behind the CLS slot of every sample
+
+
+@pytest.fixture(scope="module")
+def sres():
+    g = torch.Generator().manual_seed(23)
+    n = 64
+    rows = SR_B * (SR_S - 1)
+    rs = (torch.rand(SR_B * SR_S, generator=g) < 0.7).float() / 0.7      # drop-path keep mask / keep prob, per dx row
+    return dict(dx=torch.randn(SR_B * SR_S, n, generator=g), o=torch.randn(rows, n, generator=g).bfloat16(),
+                gamma=torch.randn(n, generator=g), rs_long=rs, rows=rows)
+
+
+def sres_outputs(d, mutation=None):
+    rows = d["rows"]
+    idx = R.scale_resid_rows(rows, SR_S, SR_S - 1, 1)
+    rs = d["rs_long"][:rows]
+    got_idx = idx - 1 if mutation == "in_shift_off_by_one" else idx
+    got_rs = d["rs_long"][idx] if mutation == "row_scale_by_input_row" else rs
+    dd = got_rs[:, None] * d["dx"][got_idx] * d["gamma"]
+    dg, _ = _partials(got_rs[:, None] * d["dx"][got_idx] * d["o"].float(), min(rows, 1056))
+    db, _ = _partials(dd, min(rows, 1056))
+    r = R.scale_resid_bwd_ref(d["dx"][idx], d["o"], d["gamma"], rs)
+    return {"d_o": (dd.bfloat16(), r.d_o, r.d_o_err, torch.bfloat16), "dgamma": (dg, r.dgamma, r.dgamma_err, torch.float32),
+            "dbias": (db, r.dbias, r.dbias_err, torch.float32)}
+
+
+def misc_outputs(mutation=None):
+    """l2_normalize_bwd, text_embed_bwd, geglu fwd / bwd and ln_fold, each emulated in fp32"""
+    g = torch.Generator().manual_seed(29)
+    res = {}
+    x, dy = torch.randn(40, 96, generator=g) * 3, torch.randn(40, 96, generator=g)
+    nrm = torch.sqrt((x * x).sum(1, keepdim=True))
+    inv = 1.0 / nrm
+    k = (x * dy).sum(1, keepdim=True) * inv * inv * inv
+    v = dy * inv - (0.0 if mutation == "l2_no_projection" else x * k)
+    ref, bnd = R.l2_normalize_bwd_ref(x, dy)
+    res["l2_dx"] = (v, ref, bnd, torch.float32)
+    # text_embed_bwd: B = 4 texts of T = 12 tokens, pad id 1 at the end of three of them; vocabulary of 9 (many duplicates)
+    B, T, D, V = 4, 12, 32, 9
+    tok = torch.randint(2, V, (B, T), generator=g)
+    for b, p in enumerate((12, 7, 3, 10)):
+        tok[b, p:] = 1
+    dxe = torch.randn(B, T + 1, D, generator=g)
+    t0, p0, c0 = torch.randn(V, D, generator=g), torch.randn(T + 1, D, generator=g), torch.randn(D, generator=g)
+    live = (tok != 1) | (mutation == "pad_not_skipped")
+    dt, dp = t0.clone(), p0.clone()
+    bi, si = live.nonzero(as_tuple=True)
+    dt.index_add_(0, tok[bi, si], dxe[bi, si + 1])
+    dp.index_add_(0, si + 1, dxe[bi, si + 1])
+    dp[0] += dxe[:, 0].sum(0)
+    ok = (tok != 1)
+    bi, si = ok.nonzero(as_tuple=True)
+    res["dtable"] = (dt, *R.scatter_ref(t0, tok[bi, si], dxe[bi, si + 1]), torch.float32)
+    dest = torch.cat([torch.zeros(B, dtype=torch.long), si + 1])
+    res["dpos"] = (dp, *R.scatter_ref(p0, dest, torch.cat([dxe[:, 0], dxe[bi, si + 1]])), torch.float32)
+    # geglu
+    gl = (torch.randn(64, 2 * 128, generator=g) * 3).bfloat16()
+    du = torch.randn(64, 128, generator=g).bfloat16()
+    a, b = gl.double()[:, :128], gl.double()[:, 128:]
+    if mutation == "geglu_halves_swapped":
+        a, b = b, a
+    u = (gelu_erf(a) * b).float()
+    res["geglu_u"] = (u.bfloat16(), *R.geglu_ref(gl), torch.bfloat16)
+    dgl = torch.cat([_f32(_f32(du.double() * b) * gelu_grad(a)), _f32(du.double() * gelu_erf(a))], 1).float()
+    res["geglu_dgl"] = (dgl.bfloat16(), *R.geglu_bwd_ref(gl, du), torch.bfloat16)
+    # ln_fold with the GeGLU interleave: 256 weight rows (two 128-row halves of wi_0), K = 200
+    W = torch.randn(256, 200, generator=g) * 0.05
+    lw, lb, bias = 1 + 0.2 * torch.randn(200, generator=g), 0.1 * torch.randn(200, generator=g), torch.randn(256, generator=g)
+    f = R.ln_fold_ref(W, lw, lb, bias, interleave=1)
+    wg = (W * lw).bfloat16()
+    dest = f.rows + (128 if mutation == "interleave_wi1_first" else 0)
+    buf_cs, buf_b = torch.zeros(512), torch.zeros(512)
+    buf_cs[dest] = wg.float().sum(1)
+    buf_b[dest] = (W * lb).sum(1) + bias
+    res["fold_wg"] = (wg.float(), f.wg.double(), torch.zeros(256, 200, dtype=torch.float64), torch.float32)
+    res["fold_colsum"] = (buf_cs[f.rows], f.colsum, f.colsum_err, torch.float32)
+    res["fold_bias"] = (buf_b[f.rows], f.bias, f.bias_err, torch.float32)
+    return res
+
+
+ROW_MUTATIONS = {
+    "neighbour_row_stats": "ln_bwd", "drop_xhat_term": "ln_bwd", "gamma_after_sums": "ln_bwd", "unshifted_var": "ln_bwd",
+    "last_partial_dropped": "ln_bwd", "merge_xy_swapped": "ln_fwd", "in_shift_off_by_one": "sres",
+    "row_scale_by_input_row": "sres", "l2_no_projection": "misc", "pad_not_skipped": "misc",
+    "geglu_halves_swapped": "misc", "interleave_wi1_first": "misc"}
+
+
+def row_outputs(kind, rowk, sres, mutation=None):
+    if kind == "ln_bwd":
+        return ln_bwd_outputs(rowk, False, mutation)
+    if kind == "ln_bwd_gelu":
+        return ln_bwd_outputs(rowk, True, mutation)
+    if kind == "ln_fwd":
+        return ln_fwd_outputs(rowk, mutation)
+    if kind == "sres":
+        return sres_outputs(sres, mutation)
+    return misc_outputs(mutation)
+
+
+@pytest.mark.parametrize("kind", ["ln_bwd", "ln_bwd_gelu", "ln_fwd", "sres", "misc"])
+def test_row_emulation_passes(rowk, sres, kind):
+    for name, (got, ref, bound, dt) in row_outputs(kind, rowk, sres).items():
+        r = R.assert_within(got, ref, bound, 1.0, dt, what=f"{kind} {name}")
+        print(f"{kind} {name}: {r:.3g} of the bound")
+
+
+@pytest.mark.parametrize("mutation", list(ROW_MUTATIONS))
+def test_row_mutation_fails(rowk, sres, mutation):
+    """each mistake exceeds the bound at least ten-fold on at least one output (run with -s to see the factors)"""
+    ratios = {name: _ratio(*v) for name, v in row_outputs(ROW_MUTATIONS[mutation], rowk, sres, mutation).items()}
+    name = max(ratios, key=ratios.get)
+    print(f"{mutation}: {name} exceeds its bound {ratios[name]:.3g}-fold")
+    assert ratios[name] >= 10, ratios
