@@ -12,7 +12,10 @@
 // parts").  Each thread reads the bias of its two query rows straight from the fp32 table (L2 resident) or gathers
 // it from the LUT.  Warps whose 16 query rows are all >= S and key n-tiles / k-steps that are all >= S are skipped
 // (S = 197 = 3*64 + 5 leaves mostly-empty edge tiles).
+//
+// Sequences of at most kAttnShortMaxS tokens run on the wgmma kernel of attention_wgmma.cu instead (see launch_fwd).
 #include "common.cuh"
+#include "ops.h"
 
 namespace opb {
 
@@ -54,15 +57,6 @@ struct AttnSmem {
 };
 static_assert(sizeof(AttnSmem) <= 48 * 1024, "launched without an opt-in for more dynamic shared memory");
 
-// LUT form of the relative-position bias: bias[h][i][j] = lut[h][code_row[i] - code_col[j]] (see kernels.RelPosBias), zero
-// between the two modality segments [0, seg_split) / [seg_split, S) of a concatenated sequence when seg_split > 0.
-struct LutBias {
-  const float* lut = nullptr;
-  int lut_len = 0;
-  const int* code_row = nullptr;
-  const int* code_col = nullptr;
-  int seg_split = 0;
-};
 OPB_DEVICE float lut_bias(const LutBias& lb, const float* lut_h, int crow, int qrow, int key, int S) {
   if (qrow >= S || key >= S || (lb.seg_split > 0 && ((qrow < lb.seg_split) != (key < lb.seg_split)))) return 0.f;
   return lut_h[crow - lb.code_col[key]];
@@ -294,6 +288,8 @@ static int launch_fwd(const void* qkv, const float* bias, const uint8_t* key_pad
                       int B, int S, int H, int s_pad, long bias_bstride, const LutBias& lb, cudaStream_t stream) {
   if (B <= 0 || S <= 0 || H <= 0) return OPB_ERR_INVALID;
   if (bias != nullptr && (s_pad < S || (s_pad & 3))) return OPB_ERR_INVALID;
+  if (S <= kAttnShortMaxS && lb.lut_len <= kAttnShortMaxLut)
+    return attention_fwd_short(qkv, bias, key_pad, out, lse, ln_stats, B, S, H, s_pad, bias_bstride, lb, stream);
   const int q_chunks = (S + kQTile - 1) / kQTile;
   const long grid = static_cast<long>(H) * q_chunks * B;
   attention_fwd_kernel<<<static_cast<unsigned>(grid), 128, sizeof(AttnSmem), stream>>>(

@@ -93,6 +93,45 @@ OPB_DEVICE void mbar_wait(uint64_t* bar, uint32_t parity) {
   }
 }
 
+// Bounded wait without mbar_wait's printf: a function call anywhere in a kernel makes ptxas serialise its wgmma pipeline
+OPB_DEVICE void mbar_wait_quiet(uint64_t* bar, uint32_t parity) {
+  if (mbar_try_wait(bar, parity)) return;
+  const uint64_t t0 = globaltimer_ns();
+  while (!mbar_try_wait(bar, parity)) {
+    if (globaltimer_ns() - t0 > OPB_WATCHDOG_NS) __trap();
+  }
+}
+
+// ----------------------------------------------------------------------------------------------
+// wgmma
+// ----------------------------------------------------------------------------------------------
+// Shared-memory matrix descriptor (sm_90), 128-byte swizzle.  K-major: rows of 128 B, 8-row groups SBO = 1024 B apart (LBO
+// unused).  MN-major: atoms of 64 MN elements x 8 k-rows (1024 B), k groups SBO = 1024 B apart, 64-wide MN chunks LBO apart.
+OPB_DEVICE uint64_t wgmma_desc_sw128(uint32_t smem_addr, uint32_t lbo) {
+  uint64_t d = 0;
+  d |= static_cast<uint64_t>((smem_addr & 0x3FFFFu) >> 4);
+  d |= static_cast<uint64_t>((lbo >> 4) & 0x3FFFu) << 16;
+  d |= static_cast<uint64_t>(1024 >> 4) << 32;
+  d |= static_cast<uint64_t>(1) << 62;   // layout type 1 = SWIZZLE_128B
+  return d;
+}
+
+OPB_DEVICE void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+OPB_DEVICE void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+OPB_DEVICE void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+
+// SM count of the current device, queried once per translation unit (persistent grids)
+static inline int sm_count() {
+  static int n = 0;
+  if (n == 0) {
+    int dev = 0;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
+  }
+  return n;
+}
+
 // ----------------------------------------------------------------------------------------------
 // TMA (cp.async.bulk.tensor) — 2D tiles global -> shared
 // ----------------------------------------------------------------------------------------------

@@ -1,5 +1,6 @@
 // Internal (C++) interface of the wgmma GEMM; the C-ABI wrappers live in c_abi.cu.
 #pragma once
+#include <cuda.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -78,6 +79,11 @@ int gemm_bf16_t(const void* A, int lda, int a_mn, const void* B, int ldb, int b_
 // Grouped "sliding window" GEMM = grouped Conv1d over channel-last activations:
 //   out[r, g*n_per_group + n] = epilogue( sum_{j < taps} sum_{c < c_pad} X[(r + j), g, c] * W[g*n_per_group + n, j*c_pad + c] )
 // X is bf16 [rows + taps - 1, groups, c_pad] (c_pad a multiple of 64), W is bf16 [groups*n_per_group, taps*c_pad].
+// TMA map of a batch of bf16 row-major matrices (csrc/attention_wgmma.cu): dims {cols, rows, batches}, pitches ld and
+// batch_stride (elements), box = 64 cols x box_rows x 1 with the 128-byte swizzle.
+int make_tmap_bf16_batched(CUtensorMap* out, const void* ptr, uint64_t cols, uint64_t rows, uint64_t ld, uint64_t batches,
+                           uint64_t batch_stride, uint32_t box_rows);
+
 int gemm_bf16_grouped_window(const void* X, const void* W, int rows, int groups, int c_pad, int taps, int n_per_group,
                              int epi, const GemmEpilogue& ep, cudaStream_t stream);
 

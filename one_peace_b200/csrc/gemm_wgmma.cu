@@ -70,23 +70,8 @@ struct GemmGeom {
 };
 
 // ----------------------------------------------------------------------------------------------
-// wgmma helpers
+// wgmma helpers (descriptor, fence / commit / wait: common.cuh)
 // ----------------------------------------------------------------------------------------------
-// Shared-memory matrix descriptor (sm_90), 128-byte swizzle.  K-major: rows of 128 B, 8-row groups SBO = 1024 B apart (LBO
-// unused).  MN-major: atoms of 64 MN elements x 8 k-rows (1024 B), k groups SBO = 1024 B apart, 64-wide MN chunks LBO apart.
-OPB_DEVICE uint64_t wgmma_desc_sw128(uint32_t smem_addr, uint32_t lbo) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((smem_addr & 0x3FFFFu) >> 4);
-  d |= static_cast<uint64_t>((lbo >> 4) & 0x3FFFu) << 16;
-  d |= static_cast<uint64_t>(1024 >> 4) << 32;
-  d |= static_cast<uint64_t>(1) << 62;   // layout type 1 = SWIZZLE_128B
-  return d;
-}
-
-OPB_DEVICE void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
-OPB_DEVICE void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
-template <int N>
-OPB_DEVICE void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 // keeps the compiler from moving accumulator reads / writes across the asynchronous wgmma window
 OPB_DEVICE void fence_acc(float (&d)[128]) {
 #pragma unroll
@@ -163,16 +148,6 @@ OPB_DEVICE float2 ldf2(const float* p) { return *reinterpret_cast<const float2*>
 OPB_DEVICE float quad_sum(float v) {
   v += __shfl_xor_sync(0xffffffffu, v, 1);
   return v + __shfl_xor_sync(0xffffffffu, v, 2);
-}
-
-// Bounded wait (common.cuh's mbar_wait without its printf: a function call anywhere in the kernel makes ptxas serialise the
-// wgmma pipeline)
-OPB_DEVICE void mbar_wait_quiet(uint64_t* bar, uint32_t parity) {
-  if (mbar_try_wait(bar, parity)) return;
-  const uint64_t t0 = globaltimer_ns();
-  while (!mbar_try_wait(bar, parity)) {
-    if (globaltimer_ns() - t0 > OPB_WATCHDOG_NS) __trap();
-  }
 }
 
 // One tile's k-blocks.  `it0` counts the k-blocks this CTA consumed for earlier tiles: the stage ring and its phases run on
@@ -676,14 +651,23 @@ int make_tmap_bf16_3d(CUtensorMap* out, const void* ptr, uint64_t k_inner, uint6
   return r == CUDA_SUCCESS ? OPB_OK : OPB_ERR_CUDA;
 }
 
-static int sm_count() {
-  static int n = 0;
-  if (n == 0) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-  }
-  return n;
+// 3D view of a batch of row-major matrices: dims {cols, rows, batches}; element (c, r, b) lives at
+// ptr + b*batch_stride + r*ld + c.  box = 64 cols x box_rows x 1, 128B swizzle; rows >= `rows` of a box are zero-filled,
+// so a box never reads into the next matrix of the batch.
+int make_tmap_bf16_batched(CUtensorMap* out, const void* ptr, uint64_t cols, uint64_t rows, uint64_t ld, uint64_t batches,
+                           uint64_t batch_stride, uint32_t box_rows) {
+  PFN_encodeTiled enc = get_encode_fn();
+  if (enc == nullptr) return OPB_ERR_CUDA;
+  if ((reinterpret_cast<uintptr_t>(ptr) & 15) != 0 || (ld * 2) % 16 != 0 || (batch_stride * 2) % 16 != 0)
+    return OPB_ERR_INVALID;
+  cuuint64_t gdim[3] = {cols, rows, batches};
+  cuuint64_t gstride[2] = {ld * 2, batch_stride * 2};
+  cuuint32_t box[3] = {static_cast<cuuint32_t>(kBlockK), box_rows, 1};
+  cuuint32_t estr[3] = {1, 1, 1};
+  CUresult r = enc(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<void*>(ptr), gdim, gstride, box, estr,
+                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  return r == CUDA_SUCCESS ? OPB_OK : OPB_ERR_CUDA;
 }
 
 template <int EPI>

@@ -10,6 +10,22 @@ int attention_fwd(const void* qkv, const float* bias, const uint8_t* key_pad, vo
 int attention_lut_fwd(const void* qkv, const float* lut, int lut_len, const int* code_row, const int* code_col,
                       const uint8_t* key_pad, void* out, float* lse, float* ln_stats, int B, int S, int H, int seg_split,
                       cudaStream_t stream);
+// LUT form of the relative-position bias: bias[h][i][j] = lut[h][code_row[i] - code_col[j]] (see kernels.RelPosBias), zero
+// between the two modality segments [0, seg_split) / [seg_split, S) of a concatenated sequence when seg_split > 0.
+struct LutBias {
+  const float* lut = nullptr;
+  int lut_len = 0;
+  const int* code_row = nullptr;
+  const int* code_col = nullptr;
+  int seg_split = 0;
+};
+// Short-sequence forward (csrc/attention_wgmma.cu): wgmma, one (sample, head) per work unit with the whole key row in
+// registers.  attention_fwd / attention_lut_fwd dispatch to it for S <= kAttnShortMaxS when the LUT row (if any) fits its
+// shared-memory slot; arguments as launch_fwd in attention.cu.
+constexpr int kAttnShortMaxS = 224;
+constexpr int kAttnShortMaxLut = 4096;
+int attention_fwd_short(const void* qkv, const float* bias, const uint8_t* key_pad, void* out, float* lse, float* ln_stats,
+                        int B, int S, int H, int s_pad, long bias_bstride, const LutBias& lb, cudaStream_t stream);
 int relpos_lut_build(const float* table, const int* idx, float* lut, int L, int H, cudaStream_t stream);
 int ln_stats_finalize(const float* partial, int parts, int rows, int dim, float eps, float* mu, float* rstd,
                       cudaStream_t stream);

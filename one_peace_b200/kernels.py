@@ -74,7 +74,7 @@ def gemm(a, w, epi, out, *, bias=None, colscale=None, gamma=None, resid=None, ou
 
 class RelPosBias:
     """Relative-position bias of one forward in both forms the attention kernels take: the dense fp32 (H,S,S_pad)
-    table (mma.sync kernel, any S) and the LUT form (same kernel; the adapters build it for S <= ATTN_TC_MAX_S)."""
+    table (any S) and the LUT form (same kernels; the adapters build it for S <= ATTN_TC_MAX_S)."""
 
     def __init__(self, dense=None, lut=None, code_row=None, code_col=None, seg_split=0):
         self.dense, self.lut, self.code_row, self.code_col, self.seg_split = dense, lut, code_row, code_col, seg_split
@@ -115,7 +115,7 @@ ATTN_TC_MAX_S = 384
 
 
 def attention_tc(qkv, rp, key_pad, B, S, H, out=None, ln_stats=None, lse=None):
-    """attention with the LUT-form bias (any S; the kernel reads the LUT from global memory).  rp: RelPosBias with the LUT form
+    """attention with the LUT-form bias (any S; for S <= 224 the kernel stages the head's LUT row in shared memory).  rp: RelPosBias with the LUT form
     (rp.seg_split > 0: two concatenated modalities, block-diagonal bias; S <= 384 then)."""
     D = H * 64
     assert qkv.dtype == torch.bfloat16 and qkv.shape == (B * S, 3 * D) and qkv.is_contiguous()
@@ -185,7 +185,8 @@ def ln_stats_finalize(partial, parts, rows, dim, eps, mu, rstd):
 
 
 def attention(qkv, bias, key_pad, B, S, H, out=None, lse=None, ln_stats=None):
-    """mma.sync attention, any S.  bias: dense fp32 (H,S,S_pad) shared by the batch, or (B,H,S,S_pad) per sample."""
+    """attention, any S (wgmma kernel for S <= 224, mma.sync above).  bias: dense fp32 (H,S,S_pad) shared by the batch, or
+    (B,H,S,S_pad) per sample."""
     _need_cuda(qkv, bias, key_pad)
     D = H * 64
     assert qkv.dtype == torch.bfloat16 and qkv.shape == (B * S, 3 * D) and qkv.is_contiguous()

@@ -3,7 +3,10 @@
     LUT form (the form the adapters use for S <= 384), outputs compared;
   * backward at the same shape with the dense bias / dbias tables and with the transposed tables the training stack uses
     (S <= 224), input gradients compared;
-  * forward of 15 s audio (B=16, S=750) with the dense bias.
+  * forward of 15 s audio (B=16, S=750) with the dense bias;
+  * the call the inference stack makes (LUT form, ln_stats, no lse) at B=64 for S=33 (text), 197 (image) and 214 (text +
+    image, two-segment LUT), with the rate against the bytes the algorithm has to move (qkv read, bf16 output and ln_stats
+    records written).
 usage: python scripts/bench_attention.py"""
 import json
 import sys
@@ -66,4 +69,26 @@ ba = R.make_token_bucket_position(256)[:Sa, :Sa]
 da = K.relpos_bias_build(torch.randn(514, H, device="cuda", generator=g), ba.cuda(), Sa, H)
 oa = torch.empty(Ba * Sa, D, dtype=torch.bfloat16, device="cuda")
 res["fwd_audio_750_us"] = timeit(lambda: K.attention(qa, da, None, Ba, Sa, H, out=oa))
+
+
+def stack_fwd(Sx, rpx):
+    """LUT form with ln_stats and without lse, as the encoder stack calls it; us per launch and GB/s of algorithmic bytes"""
+    qx = (torch.randn(B * Sx, 3 * D, device="cuda", generator=g) * 0.5).bfloat16()
+    ox = torch.empty(B * Sx, D, dtype=torch.bfloat16, device="cuda")
+    st = torch.empty(H * B * Sx * 2, device="cuda")
+    us = timeit(lambda: K.attention_tc(qx, rpx, None, B, Sx, H, out=ox, ln_stats=st))
+    nbytes = qx.numel() * 2 + ox.numel() * 2 + st.numel() * 4
+    return {"us": us, "MB": round(nbytes / 1e6, 1), "GB_per_s": round(nbytes / us / 1e3, 1)}
+
+
+def text_lut(Sx):
+    li = relpos.build_lut_index(R.make_token_bucket_position(256)[:Sx, :Sx].numpy(), relpos.text_codes(Sx))
+    return li, K.RelPosBias(lut=K.relpos_lut_build(torch.randn(514, H, device="cuda", generator=g), torch.from_numpy(li[0]).cuda()),
+                            code_row=torch.from_numpy(li[1]).cuda(), code_col=torch.from_numpy(li[2]).cuda())
+
+
+res["fwd_stack_us"] = {"S33_text": stack_fwd(33, text_lut(33)[1]), "S197_image": stack_fwd(S, rp)}
+li17 = text_lut(17)[0]
+rp214 = K.build_segmented_lut([(torch.randn(514, H, device="cuda", generator=g), li17, 17), (table, li, S)], "cuda")
+res["fwd_stack_us"]["S214_two_segment"] = stack_fwd(17 + S, rp214)
 print(json.dumps(res), flush=True)
