@@ -449,6 +449,42 @@ int opb_gemm_bf16_t(const void* A, int64_t lda, int a_mn, const void* B, int64_t
 int opb_ln_fold(const void* W, int w_dtype, int64_t ldw, const float* ln_weight, const float* ln_bias, const float* bias_in,
                 int N, int K, int interleave, void* out_w, int64_t ldo, float* colsum, float* bias_out, void* stream);
 
+/* ------------------------------------------------------------------------------------------------------------------
+ * Classification head of one_peace_classify.
+ *   opb_attn_pool_fwd : MultiheadAttentionPooling (models/one_peace/one_peace_base.py:146-173) after its k/v projection: per
+ *                       sample b and head h, s_j = q[h] . k[b,j,h] (q NOT scaled), p = softmax_j(s) in fp32 over the keys with
+ *                       key_pad[b,j] == 0, out[b, h*64:(h+1)*64] = bf16(sum_j p_j v[b,j,h]), lse[b*H + h] = log sum_j e^s_j.
+ *                       kv bf16 [B, T, 2d] (k in columns [0, d), v in [d, 2d)), q fp32 [H, 64], key_pad uint8 [B, T] or NULL,
+ *                       out bf16 [B, d], lse fp32 [B, H]; H = d / 64, any T >= 1.  Padded key rows are never read.  A sample
+ *                       whose keys are all padded gets out = 0 and lse = -inf (the reference produces NaN there).
+ *   opb_attn_pool_bwd : its adjoint for dout bf16 [B, d]: dkv bf16 [B, T, 2d] with dk[b,j,h] = p_j (dout[b,h] . v_j - delta) q[h],
+ *                       dv[b,j,h] = p_j dout[b,h]; padded key rows are written as exact zeros.  dq fp32 [H, 64] = sum_b sum_j
+ *                       ds_j k_j through the per-(b, h) partials dq_ws fp32 [B, H, 64] (caller-allocated scratch) summed over b in
+ *                       order: no atomics, repeat launches are bit-identical.
+ * ------------------------------------------------------------------------------------------------------------------ */
+int opb_attn_pool_fwd(const void* kv, const float* q, const uint8_t* key_pad, void* out, float* lse, int B, int T, int d,
+                      void* stream);
+int opb_attn_pool_bwd(const void* kv, const float* q, const uint8_t* key_pad, const float* lse, const void* dout, void* dkv,
+                      float* dq_ws, float* dq, int B, int T, int d, void* stream);
+
+/*
+ * Classification criteria (criterions/classify_loss.py:48-64 and criterions/hinge_loss.py:41-53), forward and the gradient of a
+ * unit upstream gradient in one launch.  logits fp32 [rows, ld], of which the first n_valid columns are classes (the rest is
+ * the padding of the classifier GEMM to N % 8 == 0 and is never read).  mode:
+ *   0  hard labels int64 [rows]: cross_entropy(label_smoothing = eps); n_correct = (argmax == label), first index on ties; a
+ *      label outside [0, n_valid) contributes nothing (ignore_index);
+ *   1  soft targets fp32 [rows, ld_t]: -(targets * log_softmax).sum(); n_correct = (softmax * targets).sum(); eps unused;
+ *   2  multi-label targets fp32 [rows, ld_t]: binary_cross_entropy_with_logits; n_correct = targets[argmax];
+ *   3  hinge over groups of num_choices rows (n_valid == 1, labels int64 [rows / num_choices]): sum_c max(0, 1 + z_c - z_label),
+ *      the positive's own term included; n_correct = (argmax == label).
+ * Writes row_loss / row_correct fp32 [rows] ([rows / num_choices] for mode 3), dlogits fp32 [rows, ld] (zero in the padding
+ * columns) and out2 = {sum of row_loss, sum of row_correct}, summed in a fixed order by the last CTA to finish.  ticket: one
+ * zero-initialised uint32, left at zero.
+ */
+int opb_classify_loss(const float* logits, int64_t ld, int rows, int n_valid, int mode, const int64_t* labels,
+                      const float* targets, int64_t ld_t, float eps, int num_choices, float* row_loss, float* dlogits,
+                      float* row_correct, float* out2, unsigned int* ticket, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

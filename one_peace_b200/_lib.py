@@ -98,6 +98,11 @@ SIGNATURES.update({
                                 c_void_p, c_int, c_void_p]),
     "opb_ln_fold": (c_int, [c_void_p, c_int, c_int64, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_int64,
                             c_void_p, c_void_p, c_void_p]),
+    "opb_attn_pool_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
+    "opb_attn_pool_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int,
+                                  c_int, c_void_p]),
+    "opb_classify_loss": (c_int, [c_void_p, c_int64, c_int, c_int, c_int, c_void_p, c_void_p, c_int64, c_float, c_int, c_void_p,
+                                  c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
 })
 
 

@@ -414,4 +414,24 @@ int opb_ln_fold(const void* W, int w_dtype, int64_t ldw, const float* ln_weight,
                       static_cast<cudaStream_t>(stream));
 }
 
+int opb_attn_pool_fwd(const void* kv, const float* q, const uint8_t* key_pad, void* out, float* lse, int B, int T, int d,
+                      void* stream) {
+  if (!kv || !q || !out || !lse) return OPB_ERR_INVALID;
+  return opb::attn_pool_fwd(kv, q, key_pad, out, lse, B, T, d, static_cast<cudaStream_t>(stream));
+}
+
+int opb_attn_pool_bwd(const void* kv, const float* q, const uint8_t* key_pad, const float* lse, const void* dout, void* dkv,
+                      float* dq_ws, float* dq, int B, int T, int d, void* stream) {
+  if (!kv || !q || !lse || !dout || !dkv || !dq_ws || !dq) return OPB_ERR_INVALID;
+  return opb::attn_pool_bwd(kv, q, key_pad, lse, dout, dkv, dq_ws, dq, B, T, d, static_cast<cudaStream_t>(stream));
+}
+
+int opb_classify_loss(const float* logits, int64_t ld, int rows, int n_valid, int mode, const int64_t* labels,
+                      const float* targets, int64_t ld_t, float eps, int num_choices, float* row_loss, float* dlogits,
+                      float* row_correct, float* out2, unsigned int* ticket, void* stream) {
+  if (!logits || !row_loss || !dlogits || !row_correct || !out2 || !ticket) return OPB_ERR_INVALID;
+  return opb::classify_loss(logits, ld, rows, n_valid, mode, labels, targets, ld_t, eps, num_choices, row_loss, dlogits,
+                            row_correct, out2, ticket, static_cast<cudaStream_t>(stream));
+}
+
 }  // extern "C"

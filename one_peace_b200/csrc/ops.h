@@ -149,4 +149,13 @@ int ln_fold(const void* W, int w_dtype, long ldw, const float* g, const float* b
 int topk10_rows(const float* sim, long ld, int* idx, float* val, int R, int C, cudaStream_t stream);
 int recall_hits(const int* idx, const int64_t* cand_ids, const int64_t* row_ids, int R, int* hits3, cudaStream_t stream);
 
+// csrc/classify.cu: attention pooling of the classification head and the classification criteria
+int attn_pool_fwd(const void* kv, const float* q, const uint8_t* key_pad, void* out, float* lse, int B, int T, int d,
+                  cudaStream_t stream);
+int attn_pool_bwd(const void* kv, const float* q, const uint8_t* key_pad, const float* lse, const void* dout, void* dkv,
+                  float* dq_ws, float* dq, int B, int T, int d, cudaStream_t stream);
+int classify_loss(const float* logits, long ld, int rows, int n_valid, int mode, const int64_t* labels, const float* targets,
+                  long ld_t, float eps, int num_choices, float* row_loss, float* dlogits, float* row_correct, float* out2,
+                  unsigned int* ticket, cudaStream_t stream);
+
 }  // namespace opb

@@ -50,6 +50,10 @@ except Exception:  # ImportError or transitive failures (omegaconf, hydra ...)
         def log_scalar(*a, **k):
             pass
 
+        @staticmethod
+        def log_derived(*a, **k):
+            pass
+
     metrics = _Metrics()
 
     def _register(name, dataclass=None):

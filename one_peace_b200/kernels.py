@@ -786,3 +786,73 @@ def gemm_t(a, b, epi, out, a_mn=False, b_mn=False, bias=None, cta_group=0):
     if PROFILE_HOOK is not None:
         PROFILE_HOOK("gemm", 2.0 * M * N * Kd, (M, N, Kd, epi))
     return out
+
+
+# ----------------------------------------------------------------------------------------------------------------
+# classification head (csrc/classify.cu)
+# ----------------------------------------------------------------------------------------------------------------
+def attn_pool_fwd(kv, q, key_pad, B, T):
+    """kv bf16 [B*T, 2d] (k | v), q fp32 [H, 64], key_pad uint8 [B, T] or None -> (out bf16 [B, d], lse fp32 [B, H])."""
+    _need_cuda(kv, q, key_pad)
+    d = kv.shape[1] // 2
+    assert kv.dtype == torch.bfloat16 and kv.is_contiguous() and kv.shape[0] == B * T
+    assert q.dtype == torch.float32 and q.is_contiguous() and q.numel() == d
+    if key_pad is not None:
+        assert key_pad.dtype == torch.uint8 and key_pad.shape == (B, T) and key_pad.is_contiguous()
+    out = torch.empty(B, d, dtype=torch.bfloat16, device=kv.device)
+    lse = torch.empty(B, d // 64, dtype=torch.float32, device=kv.device)
+    st = _lib.load().opb_attn_pool_fwd(kv.data_ptr(), q.data_ptr(), _ptr(key_pad), out.data_ptr(), lse.data_ptr(), B, T, d,
+                                       _stream())
+    _lib.check(st, "opb_attn_pool_fwd")
+    _count()
+    return out, lse
+
+
+def attn_pool_bwd(kv, q, key_pad, lse, dout, B, T):
+    """Adjoint of attn_pool_fwd for dout bf16 [B, d] -> (dkv bf16 [B*T, 2d], dq fp32 [H, 64])."""
+    _need_cuda(kv, q, key_pad, lse, dout)
+    d = kv.shape[1] // 2
+    assert dout.dtype == torch.bfloat16 and dout.is_contiguous() and dout.shape == (B, d)
+    assert lse.dtype == torch.float32 and lse.is_contiguous() and lse.shape == (B, d // 64)
+    if key_pad is not None:
+        assert key_pad.dtype == torch.uint8 and key_pad.shape == (B, T) and key_pad.is_contiguous()
+    dkv = torch.empty_like(kv)
+    ws = torch.empty(B, d, dtype=torch.float32, device=kv.device)
+    dq = torch.empty(d // 64, 64, dtype=torch.float32, device=kv.device)
+    st = _lib.load().opb_attn_pool_bwd(kv.data_ptr(), q.data_ptr(), _ptr(key_pad), lse.data_ptr(), dout.data_ptr(), dkv.data_ptr(),
+                                       ws.data_ptr(), dq.data_ptr(), B, T, d, _stream())
+    _lib.check(st, "opb_attn_pool_bwd")
+    _count(2)
+    return dkv, dq
+
+
+LOSS_HARD, LOSS_SOFT, LOSS_MULTI_LABEL, LOSS_HINGE = 0, 1, 2, 3
+_LOSS_TICKETS = {}
+
+
+def classify_loss(logits, n_valid, mode, labels=None, targets=None, eps=0.0, num_choices=1):
+    """logits fp32 [rows, >= n_valid] (unit column stride, free row pitch; columns past n_valid are never read) ->
+    (row_loss, dlogits fp32 shaped like logits' rows x pitch, row_correct, out2 = {loss sum, n_correct sum})."""
+    _need_cuda(logits, labels, targets)
+    assert logits.dtype == torch.float32 and logits.stride(1) == 1
+    rows, ld = logits.shape[0], logits.stride(0)
+    dev = logits.device
+    if targets is not None:
+        assert targets.dtype == torch.float32 and targets.stride(1) == 1
+    if labels is not None:
+        assert labels.dtype == torch.int64 and labels.is_contiguous()
+    n_out = rows // num_choices if mode == LOSS_HINGE else rows
+    row_loss = torch.empty(n_out, dtype=torch.float32, device=dev)
+    row_correct = torch.empty(n_out, dtype=torch.float32, device=dev)
+    dlogits = torch.empty(rows, ld, dtype=torch.float32, device=dev)
+    out2 = torch.empty(2, dtype=torch.float32, device=dev)
+    key = dev.index if dev.index is not None else torch.cuda.current_device()
+    if key not in _LOSS_TICKETS:
+        _LOSS_TICKETS[key] = torch.zeros(1, dtype=torch.int32, device=dev)       # the kernel leaves it at zero
+    st = _lib.load().opb_classify_loss(logits.data_ptr(), ld, rows, int(n_valid), int(mode), _ptr(labels), _ptr(targets),
+                                       targets.stride(0) if targets is not None else 0, float(eps), int(num_choices),
+                                       row_loss.data_ptr(), dlogits.data_ptr(), row_correct.data_ptr(), out2.data_ptr(),
+                                       _LOSS_TICKETS[key].data_ptr(), _stream())
+    _lib.check(st, "opb_classify_loss")
+    _count()
+    return row_loss, dlogits, row_correct, out2

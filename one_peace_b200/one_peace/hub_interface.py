@@ -6,6 +6,7 @@ part of the accelerated path: ``process_*`` delegate to user-supplied callables.
 """
 import torch
 
+from .one_peace_classify import OnePeaceClassifyConfig, OnePeaceClassifyModel
 from .one_peace_pretrain import OnePeacePretrainConfig, OnePeacePretrainModel
 from .one_peace_retrieval import OnePeaceRetrievalConfig, OnePeaceRetrievalModel
 from ..unify_model_config import one_peace_4b_decoder_config, one_peace_4b_encoder_config
@@ -28,10 +29,13 @@ class _Dictionary:
 def from_pretrained(model_name_or_path=None, model_type="one_peace_retrieval", device="cuda", dtype="float32",
                     state_dict=None, head_type="val", layers=40, embed_dim=1536, ffn_embed_dim=6144,
                     attention_heads=24, patch_image_size=256, vocab_size=50264, decoder=None, use_audio=None, use_image=True,
-                    stage2_pretrain=False):
+                    stage2_pretrain=False, num_classes=None, use_two_images=False, use_pooler=False, head_scale_ratio=1,
+                    use_image_features=False):
     """hub_interface.py:53-73.  Loads ``one-peace.pt``-style state dicts (same parameter names, strict except for
     pretraining-only keys) into the sm_90a model.  ``model_name_or_path`` may be a torch checkpoint whose
-    'model' entry is the state dict (fairseq layout) or a bare state dict; alternatively pass ``state_dict``."""
+    'model' entry is the state dict (fairseq layout) or a bare state dict; alternatively pass ``state_dict``.
+    model_type="one_peace_classify": the attention-pooling classification model of the fine-tuning recipes (head_type one of
+    text / image / audio / vl / al, `num_classes` outputs); its extract_* methods return the logits."""
     if model_type == "one_peace_pretrain":
         # models/one_peace/one_peace_pretrain.py: encoder + lightweight decoder (pretrain_vl_3B.yaml:92-168); `decoder` =
         # dict(embed_dim=, ffn_embed_dim=, layers=, attention_heads=) or None for the 4B recipe's 768 / 2048 / 2 / 12
@@ -50,15 +54,24 @@ def from_pretrained(model_name_or_path=None, model_type="one_peace_retrieval", d
         cfg.encoder = one_peace_4b_encoder_config(layers, embed_dim, ffn_embed_dim, attention_heads, patch_image_size)
         with torch.device(device):
             model = OnePeaceRetrievalModel(cfg, _Dictionary(vocab_size), head_type)
+    elif model_type == "one_peace_classify":
+        cfg = OnePeaceClassifyConfig(attn_pooling=True, use_pooler=bool(use_pooler), head_scale_ratio=head_scale_ratio,
+                                     use_image_features=bool(use_image_features))
+        cfg.encoder = one_peace_4b_encoder_config(layers, embed_dim, ffn_embed_dim, attention_heads, patch_image_size)
+        if num_classes is None:
+            raise ValueError("model_type='one_peace_classify' needs num_classes")
+        with torch.device(device):
+            model = OnePeaceClassifyModel(cfg, _Dictionary(vocab_size), head_type, num_classes, use_two_images)
     else:
-        raise NotImplementedError("model_type must be one_peace_retrieval or one_peace_pretrain (the classification heads of "
-                                  "one_peace_classify are outside the accelerated path)")
+        raise NotImplementedError("model_type must be one_peace_retrieval, one_peace_pretrain or one_peace_classify")
     if state_dict is None and model_name_or_path is not None:
         ckpt = torch.load(model_name_or_path, map_location="cpu")
         state_dict = ckpt.get("model", ckpt)
     if state_dict is not None:
         sd = dict(state_dict)
         model.upgrade_state_dict_named(sd, "")
+        if model_type == "one_peace_classify":
+            sd.pop("logit_scale", None)           # the contrastive temperature of the retrieval / pretraining checkpoints
         model.load_state_dict(sd, strict=True)
     model = model.to({"float32": torch.float32, "fp32": torch.float32, "bfloat16": torch.bfloat16,
                       "bf16": torch.bfloat16}[dtype] if isinstance(dtype, str) else dtype)
@@ -115,15 +128,35 @@ class OnePeaceHubInterface:
         return feats
 
     # -- the accelerated path (hub_interface.py:212-222) --
+    def _classify(self, **inputs):
+        """one_peace_classify: the logits (the reference's extract_text_features drops them; they are returned here)."""
+        return self.model(**{k: self._to_device(v) for k, v in inputs.items()})
+
+    def _is_classify(self):
+        return isinstance(self.model, OnePeaceClassifyModel)
+
     @torch.no_grad()
     def extract_text_features(self, src_tokens, out=None):
+        if self._is_classify():
+            return self._finish(self._classify(src_tokens=src_tokens), out)
         return self._finish(self._forward("text", src_tokens=self._to_device(src_tokens)), out)
 
     @torch.no_grad()
     def extract_image_features(self, src_images, out=None):
+        if self._is_classify():
+            return self._finish(self._classify(src_images=src_images), out)
         return self._finish(self._forward("image", src_images=self._to_device(src_images)), out)
 
     @torch.no_grad()
     def extract_audio_features(self, src_audios, audio_padding_masks, out=None):
+        if self._is_classify():
+            return self._finish(self._classify(src_audios=src_audios, audio_padding_masks=audio_padding_masks), out)
         return self._finish(self._forward("audio", src_audios=self._to_device(src_audios),
                                           audio_padding_masks=self._to_device(audio_padding_masks)), out)
+
+    @torch.no_grad()
+    def extract_vl_features(self, src_images, src_tokens, out=None):
+        """one_peace_classify with head_type 'vl' (hub_interface.py:224-225): the logits of an image-text pair."""
+        if not self._is_classify():
+            raise NotImplementedError("extract_vl_features needs model_type='one_peace_classify'")
+        return self._finish(self._classify(src_images=src_images, src_tokens=src_tokens), out)
