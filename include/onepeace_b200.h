@@ -60,6 +60,8 @@ const char* opb_status_string(int status);
  * if resid_period > 0 the residual row is (m % resid_period) + resid_row_offset (broadcast table),
  * otherwise it is out_row.  If out_group_valid > 0, rows with (m % out_group) >= out_group_valid are computed but
  * not stored (allocation slack rows of the audio frame buffers).  cta_group: 0, 1 or 2 (accepted for compatibility; every GEMM runs 128x256 tiles).
+ * resid may overlap the output only as the in-place update (resid == out, ldr == ldo, resid_period == 0) and must not
+ * overlap the bf16 copy of opb_gemm_bf16_ex; any other overlap returns OPB_ERR_INVALID before anything is launched.
  */
 int opb_gemm_bf16(const void* A, int64_t lda, const void* B, int64_t ldb, int M, int N, int K, int epi, void* out,
                   int64_t ldo, const float* bias, const float* colscale, const float* gamma, const float* resid,

@@ -23,7 +23,9 @@ struct GemmEpilogue {
   const float* bias = nullptr;     // [N] or null
   const float* colscale = nullptr; // [N] or null
   const float* gamma = nullptr;    // [N] or null (EPI_RESID_F32)
-  const float* resid = nullptr;    // fp32 residual or null (EPI_RESID_F32)
+  // fp32 residual or null (EPI_RESID_F32).  It may overlap the outputs only as the in-place update: resid == out, ldr == ldo
+  // and resid_period == 0 (anything else is refused, see resid_aliasing_ok in gemm_wgmma.cu)
+  const float* resid = nullptr;
   long ldr = 0;                    // residual row pitch
   // optional row remapping: out_row = (m / out_group) * out_group_stride + (m % out_group) + out_row_offset
   int out_group = 0;

@@ -40,6 +40,9 @@ constexpr int kThreads = 384;
 // panels and a run of weight panels, so each weight panel is read from HBM about once per band instead of once per row panel.
 // On an H100 bands of 8 and 16 time the same; bands of 1 (row-major tile order) make the GeGLU GEMM about 6 % slower.
 constexpr int kBandM = 8;
+// Column groups of the residual fragment loaded ahead of their stores in the EPI_RESID_F32 epilogue (see epilogue()): 16
+// float2 = 32 registers fit next to the 128 accumulators without spills, a whole fragment row of 32 does not.
+constexpr int kResidBatch = 16;
 
 // Epilogue operands of one tile, staged in shared memory by the spare warps of the producer warpgroup while the consumers
 // run the mainloop (two buffers: tile i + 1 is staged while tile i's epilogue reads).
@@ -337,44 +340,63 @@ OPB_DEVICE void epilogue(const float (&d)[128], const GemmEpilogue& ep, const Ge
           *reinterpret_cast<float2*>(ep.stats_out + (static_cast<long>(n_blk * 2 + 1) * M + row) * 2) = make_float2(0.f, 0.f);
         }
       } else {
+        // EPI_RESID_F32: the thread's residual fragment of this row is read in batches of kResidBatch column groups, each
+        // batch loaded before any of its stores.  `out` and `resid` may alias (the stack updates the residual stream in
+        // place), so the compiler cannot hoist a load above an earlier store: loaded inside the column loop, every column
+        // group would wait for its own global round trip.  Loading ahead is safe because an element of `resid` that is also
+        // an output element is the one this thread writes from the same fragment slot (gemm_bf16 refuses any other overlap).
 #pragma unroll
-        for (int j = 0; j < 32; ++j) {
-          const int lc = 8 * j + 2 * quad;           // column inside the tile
-          const int tc = col0 + lc;                  // column inside the group
-          if (tc >= N) continue;
-          const int col = gcol0 + tc;
-          float x0 = d[4 * j + 2 * h], x1 = d[4 * j + 2 * h + 1];
-          if (has_ln) {
-            const float2 c = ldf2(st->colsum + lc);
-            x0 = rs * (x0 - mu * c.x); x1 = rs * (x1 - mu * c.y);
-          }
-          if (ep.bias != nullptr) {
-            const float2 b = ldf2(st->bias + lc);
-            x0 += b.x; x1 += b.y;
-          }
-          if constexpr (EPI == EPI_STORE_BF16 || EPI == EPI_GELU_BF16) {
-            if (ep.colscale != nullptr) {
-              const float2 s = ldf2(st->colscale + lc);
-              x0 *= s.x; x1 *= s.y;
-            }
-            if constexpr (EPI == EPI_GELU_BF16) { x0 = gelu_erf(x0); x1 = gelu_erf(x1); }
-            if (row_ok) *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(ep.out) + out_row * ep.ldo + col) = pack_bf16x2(x0, x1);
-          } else {
-            if constexpr (EPI == EPI_RESID_F32) {
-              if (ep.gamma != nullptr) {
-                const float2 g = ldf2(st->gamma + lc);
-                x0 *= g.x; x1 *= g.y;
+        for (int jb = 0; jb < 32; jb += kResidBatch) {
+          float2 res[kResidBatch];
+          if constexpr (EPI == EPI_RESID_F32) {
+            if (ep.resid != nullptr && row_ok) {
+              const float* rp = ep.resid + res_row * ep.ldr + gcol0;
+#pragma unroll
+              for (int jj = 0; jj < kResidBatch; ++jj) {
+                const int tc = col0 + 8 * (jb + jj) + 2 * quad;
+                if (tc < N) res[jj] = ldf2(rp + tc);
               }
-              if (ep.resid != nullptr && row_ok) {
-                const float2 r = ldf2(ep.resid + res_row * ep.ldr + col);
-                x0 += r.x; x1 += r.y;
-              }
-              st_sum += x0 + x1;
-              st_sq += x0 * x0 + x1 * x1;
-              if (row_ok && ep.out_bf16 != nullptr)
-                *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(ep.out_bf16) + out_row * ep.ldo_bf16 + col) = pack_bf16x2(x0, x1);
             }
-            if (row_ok) *reinterpret_cast<float2*>(reinterpret_cast<float*>(ep.out) + out_row * ep.ldo + col) = make_float2(x0, x1);
+          }
+#pragma unroll
+          for (int jj = 0; jj < kResidBatch; ++jj) {
+            const int j = jb + jj;
+            const int lc = 8 * j + 2 * quad;           // column inside the tile
+            const int tc = col0 + lc;                  // column inside the group
+            if (tc >= N) continue;
+            const int col = gcol0 + tc;
+            float x0 = d[4 * j + 2 * h], x1 = d[4 * j + 2 * h + 1];
+            if (has_ln) {
+              const float2 c = ldf2(st->colsum + lc);
+              x0 = rs * (x0 - mu * c.x); x1 = rs * (x1 - mu * c.y);
+            }
+            if (ep.bias != nullptr) {
+              const float2 b = ldf2(st->bias + lc);
+              x0 += b.x; x1 += b.y;
+            }
+            if constexpr (EPI == EPI_STORE_BF16 || EPI == EPI_GELU_BF16) {
+              if (ep.colscale != nullptr) {
+                const float2 s = ldf2(st->colscale + lc);
+                x0 *= s.x; x1 *= s.y;
+              }
+              if constexpr (EPI == EPI_GELU_BF16) { x0 = gelu_erf(x0); x1 = gelu_erf(x1); }
+              if (row_ok) *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(ep.out) + out_row * ep.ldo + col) = pack_bf16x2(x0, x1);
+            } else {
+              if constexpr (EPI == EPI_RESID_F32) {
+                if (ep.gamma != nullptr) {
+                  const float2 g = ldf2(st->gamma + lc);
+                  x0 *= g.x; x1 *= g.y;
+                }
+                if (ep.resid != nullptr && row_ok) {
+                  x0 += res[jj].x; x1 += res[jj].y;
+                }
+                st_sum += x0 + x1;
+                st_sq += x0 * x0 + x1 * x1;
+                if (row_ok && ep.out_bf16 != nullptr)
+                  *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(ep.out_bf16) + out_row * ep.ldo_bf16 + col) = pack_bf16x2(x0, x1);
+              }
+              if (row_ok) *reinterpret_cast<float2*>(reinterpret_cast<float*>(ep.out) + out_row * ep.ldo + col) = make_float2(x0, x1);
+            }
           }
         }
         if constexpr (EPI == EPI_RESID_F32) {
@@ -704,6 +726,46 @@ static int dispatch_gemm(int epi, const CUtensorMap& ta, const CUtensorMap& tb, 
   }
 }
 
+// Bytes [begin, end) spanned by rows lo..hi of a row-major matrix with pitch ld and `cols` columns of `esz` bytes.
+struct ByteSpan {
+  const char* begin;
+  const char* end;
+};
+static ByteSpan row_span(const void* p, long lo, long hi, long ld, long cols, int esz) {
+  const char* c = static_cast<const char*>(p);
+  return {c + lo * ld * esz, c + (hi * ld + cols) * esz};
+}
+static bool spans_meet(const ByteSpan& a, const ByteSpan& b) { return a.begin < b.end && b.begin < a.end; }
+
+// The EPI_RESID_F32 epilogue loads a batch of residual values before it stores the outputs of that batch (see epilogue()).
+// That is only correct if no output store lands on a residual element that is read for another output element: `resid`
+// either lies apart from both outputs, or it is the fp32 output itself with the same pitch and row mapping (the in-place
+// update of the residual stream).
+static bool resid_aliasing_ok(const GemmEpilogue& ep, int M, long cols) {
+  if (ep.resid == nullptr) return true;
+  // output rows of rows 0..M-1: the mapping is linear in the group index and the row inside the group, so its extremes are
+  // at the corners of that grid
+  auto out_row = [&](long m) {
+    return ep.out_group > 0 ? (m / ep.out_group) * ep.out_group_stride + m % ep.out_group + ep.out_row_offset : m;
+  };
+  const long g = ep.out_group > 0 ? ep.out_group : M, last = M - 1, q = last / g;
+  const long corners[5] = {0, (g < M ? g : M) - 1, q * g, last, q > 0 ? q * g - 1 : 0};
+  long lo = out_row(0), hi = lo;
+  for (long m : corners) {
+    lo = out_row(m) < lo ? out_row(m) : lo;
+    hi = out_row(m) > hi ? out_row(m) : hi;
+  }
+  long rlo = lo, rhi = hi;
+  if (ep.resid_period > 0) {
+    rlo = ep.resid_row_offset;
+    rhi = rlo + (ep.resid_period < M ? ep.resid_period : M) - 1;
+  }
+  const ByteSpan res = row_span(ep.resid, rlo, rhi, ep.ldr, cols, 4);
+  if (ep.out_bf16 != nullptr && spans_meet(res, row_span(ep.out_bf16, lo, hi, ep.ldo_bf16, cols, 2))) return false;
+  if (!spans_meet(res, row_span(ep.out, lo, hi, ep.ldo, cols, 4))) return true;
+  return ep.resid == ep.out && ep.ldr == ep.ldo && ep.resid_period == 0;
+}
+
 static GemmGeom plain_geom(int M, int N, int K) {
   GemmGeom geo;
   geo.M = M; geo.N = N; geo.K = K;
@@ -725,6 +787,7 @@ int gemm_bf16(const void* A, int lda, const void* B, int ldb, int M, int N, int 
   if (K % 8 != 0 || N % 8 != 0 || lda % 8 != 0 || ldb % 8 != 0) return OPB_ERR_INVALID;
   if (epi == EPI_GEGLU_BF16 && N % kBlockN != 0) return OPB_ERR_INVALID;
   if (cta_group < 0 || cta_group > 2) return OPB_ERR_INVALID;
+  if (epi == EPI_RESID_F32 && !resid_aliasing_ok(ep, M, N)) return OPB_ERR_INVALID;
   GemmGeom geo = plain_geom(M, N, K);
   // Small-M split-K (a handful of texts through the 4B stack): M <= 256 gives N / 256 x 1-2 tiles, so a few CTAs would stream
   // the whole weight while the other SMs idle.  With a workspace, the fp32-residual and the plain bf16-store GEMMs instead split
@@ -780,6 +843,7 @@ int gemm_bf16_grouped_window(const void* X, const void* W, int rows, int groups,
   if (rows <= 0 || groups <= 0 || taps <= 0 || n_per_group <= 0) return OPB_ERR_INVALID;
   if (c_pad % kBlockK != 0 || n_per_group % 8 != 0 || n_per_group > kBlockN) return OPB_ERR_INVALID;
   if (epi == EPI_GEGLU_BF16 || epi == EPI_LSE_PARTIAL || epi == EPI_SOFTMAX_GRAD) return OPB_ERR_INVALID;
+  if (epi == EPI_RESID_F32 && !resid_aliasing_ok(ep, rows, static_cast<long>(groups) * n_per_group)) return OPB_ERR_INVALID;
   GemmGeom geo = plain_geom(rows, n_per_group, taps * c_pad);
   geo.kb_inner = c_pad / kBlockK;
   geo.num_k_blocks = taps * geo.kb_inner;
