@@ -152,8 +152,9 @@ int relpos_bias_build(const float* table, const int64_t* bucket, float* bias, in
   return cudaGetLastError() == cudaSuccess ? OPB_OK : OPB_ERR_CUDA;
 }
 
-// out[(b, t), j] = wav[b, 5 t + j] (j < 10), zero for j in 10..15 and for samples past the clip end;
-// rows t >= frames (allocation slack up to `pitch`) are written as zeros.
+// out[(b, t), j] = wav[b, 5 t + j] for j < 10 and 5 t + j < n_samples, zero elsewhere (j in 10..15, samples past the clip
+// end), for every t < pitch: the slack rows t >= frames hold the clip's partial last frames, which only the slack rows of
+// later layers read.
 template <typename TWav>
 __global__ void audio_frame10_kernel(const TWav* __restrict__ wav, __nv_bfloat16* __restrict__ out, int B,
                                      long n_samples, long pitch) {

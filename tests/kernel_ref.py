@@ -1,7 +1,7 @@
-"""fp64 references of the GEMM epilogues (csrc/gemm_wgmma.cu), of the contrastive-head reductions (csrc/infonce.cu), of
-the attention forward and backward (csrc/attention.cu, csrc/attention_bwd.cu) and of the row kernels (csrc/layernorm.cu,
-csrc/backward.cu, csrc/pack.cu, csrc/gather.cu), with an error bound for every output element, and NaN-canary output
-buffers.
+"""fp64 references of the GEMM epilogues (csrc/gemm_wgmma.cu) and of the convolutions lowered onto that GEMM, of the
+contrastive-head reductions (csrc/infonce.cu), of the attention forward and backward (csrc/attention.cu,
+csrc/attention_bwd.cu) and of the row kernels (csrc/layernorm.cu, csrc/backward.cu, csrc/pack.cu, csrc/gather.cu), with an
+error bound for every output element, and NaN-canary output buffers.
 
 Plain PyTorch on whatever device the inputs live on; nothing here calls the extension.
 
@@ -26,6 +26,16 @@ A kernel output ``got`` passes ``assert_within`` when, element by element,
           records (``ln_stats_ref``) and, for the contrastive head, the errors of the bf16x3 logits.
 ``u_out`` 2^-8 for a bf16 output, 0 for fp32.  Round-to-nearest to 8 significant bits moves the kernel's fp32 value v by
           less than 2^-8 |v|, and |v| exceeds |ref| by at most the fp32 error (itself far inside tau * mag).
+
+Convolutions (``window_matrix``, ``grouped_window_ref``)
+---------------------------------------------------------
+The adapters lower convolutions onto the same GEMM, and each form is the GEMM of a window matrix, so its reference is
+``gemm_ref`` on that matrix with the same bound (no new constant).  The grouped sliding window (``grouped_conv1d``) of
+group g is A_g[r, j * c_pad + c] = X[r + j, g, c] against the weight rows W[g * n : (g + 1) * n], its output the columns
+g * n ... (g + 1) * n - 1 with bias[g * n : (g + 1) * n]; every c < c_pad counts, padding channels included.  The
+reference builds one group's fp64 window at a time on the inputs' device (about 30 MB at the audio positional conv).
+Overlapping strided rows (``gemm(..., K=kw*C, lda=2*C)``, the feature-extractor convolutions) are the plain reference
+on ``flat.as_strided((M, K), (lda, 1))``; narrow K (K < 64: one zero-filled k-block) is the plain reference as is.
 
 Attention (``attention_ref``, ``attention_bwd_ref``)
 -----------------------------------------------------
@@ -245,6 +255,26 @@ def gemm_ref(a, w, epi, *, bias=None, colscale=None, gamma=None, resid=None, ln_
     if st is not None:
         ns.stats, ns.stats_mag, ns.stats_extra = st
     return ns
+
+
+def window_matrix(X, rows, groups, c_pad, taps, group):
+    """fp64 window matrix of ``group`` g in the grouped sliding-window GEMM, A_g [rows, taps * c_pad]:
+    A_g[r, j * c_pad + c] = X[r + j, g, c] for r < rows, j < taps, c < c_pad.  X holds >= rows + taps - 1 rows of
+    groups * c_pad values (any shape with that row layout)."""
+    Xg = X.reshape(-1, groups, c_pad)[:rows + taps - 1, group]
+    win = Xg.double().unfold(0, taps, 1)                 # [rows, c_pad, taps]: win[r, c, j] = X[r + j, g, c]
+    return win.transpose(1, 2).reshape(rows, taps * c_pad)
+
+
+def grouped_window_ref(X, W, rows, groups, c_pad, taps, n, epi, bias=None):
+    """fp64 result of ``grouped_conv1d``: out[:, g*n:(g+1)*n] = gemm_ref(A_g, W[g*n:(g+1)*n], epi, bias=bias[g*n:(g+1)*n]),
+    one group's window at a time.  Returns a namespace with y, mag, extra [rows, groups * n]."""
+    ys, mags, extras = [], [], []
+    for g in range(groups):
+        sl = slice(g * n, (g + 1) * n)
+        r = gemm_ref(window_matrix(X, rows, groups, c_pad, taps, g), W[sl], epi, bias=bias[sl] if bias is not None else None)
+        ys.append(r.y); mags.append(r.mag); extras.append(r.extra)
+    return SimpleNamespace(y=torch.cat(ys, 1), mag=torch.cat(mags, 1), extra=torch.cat(extras, 1))
 
 
 def assert_within(got, ref, mag, tau, out_dtype, extra=None, what="output"):

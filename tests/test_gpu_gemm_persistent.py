@@ -77,23 +77,3 @@ def test_resid_in_place_ln_partial_many_tiles(K):
     yt = y.view(M, N // 256, 256)
     torch.testing.assert_close(stats[:, :, 0], yt.sum(2).t(), atol=1e-2, rtol=1e-4)
     torch.testing.assert_close(stats[:, :, 1], (yt * yt).sum(2).t(), atol=1e-2, rtol=1e-4)
-
-
-def test_grouped_conv1d_more_tiles_than_sms(K):
-    B, T, G, cg, cpad, kp = 4, 300, 16, 24, 64, 19   # 10 row panels x 16 groups = 160 tiles
-    C = G * cg
-    halo = kp // 2
-    Tp = T + 2 * halo
-    g = torch.Generator(device="cuda").manual_seed(33)
-    x = torch.randn(B, T, C, device="cuda", generator=g)
-    w = torch.randn(C, cg, kp, device="cuda", generator=g) * 0.1
-    bias = torch.randn(C, device="cuda", generator=g)
-    buf = torch.zeros(B * Tp + kp, G, cpad, dtype=torch.bfloat16, device="cuda")
-    K.pack_group_halo(x.view(B * T, C), buf, B, T, T, 0, Tp, halo, C, cg, cpad)
-    wp = torch.zeros(C, kp, cpad, dtype=torch.bfloat16, device="cuda")
-    wp[:, :, :cg] = w.permute(0, 2, 1).bfloat16()
-    out = torch.empty(B * Tp, C, dtype=torch.float32, device="cuda")
-    K.grouped_conv1d(buf, wp.view(C, kp * cpad), bias, out, B * Tp, G, cpad, kp, cg, epi=K.EPI_STORE_F32)
-    want = torch.nn.functional.conv1d(x.bfloat16().float().transpose(1, 2), w.bfloat16().float(), bias, padding=halo,
-                                      groups=G).transpose(1, 2)
-    assert relerr(out.view(B, Tp, C)[:, :T], want) < 1e-5

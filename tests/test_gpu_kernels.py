@@ -81,20 +81,6 @@ def test_gemm_row_remap_and_broadcast_residual(K):
     assert torch.all(x[:, 0] == 7.0)       # CLS slot untouched
 
 
-def test_gemm_overlapping_strided_rows_is_conv1d(K):
-    """k=3, s=2 Conv1d over channel-last activations == GEMM on an overlapping strided view (audio.py:270-284)."""
-    T_in, C, Co = 41, 64, 128
-    T_out = (T_in - 3) // 2 + 1
-    g = torch.Generator(device="cuda").manual_seed(5)
-    x = torch.randn(T_in + 4, C, device="cuda", generator=g).bfloat16()     # + slack rows
-    w = (torch.randn(Co, C, 3, device="cuda", generator=g) * 0.1)
-    wp = w.permute(0, 2, 1).reshape(Co, 3 * C).bfloat16().contiguous()       # [out, (j, c)]
-    out = torch.empty(T_out, Co, device="cuda", dtype=torch.float32)
-    K.gemm(x, wp, K.EPI_STORE_F32, out, M=T_out, K=3 * C, lda=2 * C)
-    want = torch.nn.functional.conv1d(x[:T_in].float().t()[None], w.bfloat16().float(), stride=2)[0].t()
-    assert relerr(out, want) < 1e-5
-
-
 @pytest.mark.parametrize("B,S,H,use_bias,use_pad", [(2, 17, 4, True, True), (2, 64, 4, False, False),
                                                      (3, 197, 24, True, False), (2, 500, 4, True, True), (1, 750, 2, True, True)])
 def test_attention(K, B, S, H, use_bias, use_pad):
@@ -177,29 +163,6 @@ def test_patchify_and_l2norm(K):
     y, y16 = K.l2_normalize_rows(x.cuda(), want_bf16=True)
     torch.testing.assert_close(y.cpu(), torch.nn.functional.normalize(x, dim=1), atol=1e-6, rtol=1e-6)
     assert relerr(y16, y) < 4e-3
-
-
-def test_grouped_conv1d_matches_torch(K):
-    """Conv1d(C, C, k=19, padding=9, groups=G) on channel-last data == grouped sliding-window GEMM on the halo'd,
-    group-padded buffer (models/adapter/audio.py:57-80)."""
-    B, T, G, cg, cpad, kp = 2, 45, 4, 24, 64, 19
-    C = G * cg
-    halo = kp // 2
-    Tp = T + 2 * halo
-    g = torch.Generator(device="cuda").manual_seed(11)
-    x = torch.randn(B, T, C, device="cuda", generator=g)
-    w = torch.randn(C, cg, kp, device="cuda", generator=g) * 0.1
-    bias = torch.randn(C, device="cuda", generator=g)
-    buf = torch.zeros(B * Tp + kp, G, cpad, dtype=torch.bfloat16, device="cuda")
-    K.pack_group_halo(x.view(B * T, C), buf, B, T, T, 0, Tp, halo, C, cg, cpad)
-    wp = torch.zeros(C, kp, cpad, dtype=torch.bfloat16, device="cuda")
-    wp[:, :, :cg] = w.permute(0, 2, 1).bfloat16()
-    out = torch.empty(B * Tp, C, dtype=torch.float32, device="cuda")
-    K.grouped_conv1d(buf, wp.view(C, kp * cpad), bias, out, B * Tp, G, cpad, kp, cg, epi=K.EPI_STORE_F32)
-    want = torch.nn.functional.conv1d(x.bfloat16().float().transpose(1, 2), w.bfloat16().float(), bias, padding=halo,
-                                      groups=G).transpose(1, 2)
-    got = out.view(B, Tp, C)[:, :T]
-    assert relerr(got, want) < 1e-5
 
 
 def test_layernorm_remap_group_pad_and_accumulate(K):

@@ -169,6 +169,118 @@ def test_canary_helpers():
 
 
 # ----------------------------------------------------------------------------------------------------------------------
+# convolutions lowered onto the GEMM
+# ----------------------------------------------------------------------------------------------------------------------
+CG, CPAD, CN, CTAPS, CGROUPS, CROWS = 96, 128, 96, 19, 3, 150     # the audio positional conv's group geometry (two 64-channel
+                                                                    # k-blocks per tap), three groups
+OV_C, OV_KW, OV_M = 64, 3, 100                                      # overlapping rows: K = 3 C read at a pitch of 2 C
+
+
+@pytest.fixture(scope="module")
+def conv():
+    g = torch.Generator().manual_seed(13)
+    x = torch.zeros(CROWS + CTAPS - 1, CGROUPS, CPAD)
+    x[:, :, :CG] = torch.randn(CROWS + CTAPS - 1, CGROUPS, CG, generator=g)
+    w = torch.zeros(CGROUPS * CN, CTAPS, CPAD)
+    w[:, :, :CG] = torch.randn(CGROUPS * CN, CTAPS, CG, generator=g) * 0.05
+    K = OV_KW * OV_C
+    return dict(x=x.bfloat16(), w=w.view(CGROUPS * CN, CTAPS * CPAD).bfloat16(), bias=torch.randn(CGROUPS * CN, generator=g),
+                flat=torch.randn(OV_M * K, generator=g).bfloat16(), w_ov=(torch.randn(128, K, generator=g) * 0.05).bfloat16())
+
+
+def emulate_grouped_conv(c, mutation=None):
+    """fp32 grouped sliding-window conv as a correct kernel computes it, with an optional mistake.  Rows past the operand, a
+    group past the last and weight rows past groups * n read as zero (the tensor maps zero-fill them)."""
+    X = c["x"].float()
+    X = torch.cat([X, torch.zeros(2, CGROUPS, CPAD)], 0)
+    X = torch.cat([X, torch.zeros(X.shape[0], 1, CPAD)], 1)
+    W = torch.cat([c["w"].float(), torch.zeros(CGROUPS * 256, CTAPS * CPAD)], 0)
+    bias = torch.cat([c["bias"], torch.zeros(CN)])
+    r, j = torch.arange(CROWS)[:, None], torch.arange(CTAPS)[None, :]
+    src = r + j
+    if mutation == "tap_shift":                   # window one tap late
+        src = r + j + 1
+    if mutation == "taps_reversed":
+        src = r + (CTAPS - 1 - j)
+    out = []
+    for g in range(CGROUPS):
+        A = X[src, g + 1 if mutation == "group_c0" else g]          # [rows, taps, c_pad]; group_c0: the next group's channels
+        if mutation == "kin_swapped":             # the two 64-channel k-blocks of every tap exchanged
+            A = A.view(CROWS, CTAPS, CPAD // 64, 64).flip(2)
+        A = A.reshape(CROWS, CTAPS * CPAD)
+        w0 = g * 256 if mutation == "b_group_rows" else g * CN      # b_group_rows: a whole 256-row tile per group
+        b0 = (g + 1) * CN if mutation == "bias_neighbour" else g * CN
+        out.append(A @ W[w0:w0 + CN].t() + bias[b0:b0 + CN])
+    return torch.cat(out, 1)
+
+
+def conv_ref(c, epi=R.EPI_STORE_F32):
+    return R.grouped_window_ref(c["x"], c["w"], CROWS, CGROUPS, CPAD, CTAPS, CN, epi, bias=c["bias"])
+
+
+def overlap_ref(c):
+    K = OV_KW * OV_C
+    return R.gemm_ref(c["flat"].as_strided((OV_M, K), (2 * OV_C, 1)), c["w_ov"], R.EPI_STORE_F32)
+
+
+def emulate_overlap(c, mutation=None):
+    K = OV_KW * OV_C
+    pitch = K if mutation == "pitch_K" else 2 * OV_C
+    return c["flat"].float().as_strided((OV_M, K), (pitch, 1)) @ c["w_ov"].float().t()
+
+
+def test_window_matrix_is_conv1d():
+    """the references are Conv1d: grouped, k = 19, padding 9 on a halo'd buffer, and k = 3, stride 2 on overlapping rows"""
+    g = torch.Generator().manual_seed(17)
+    B, T, G, cg, cpad, kp = 2, 30, 3, 8, 64, 19
+    halo = kp // 2
+    x, w, b = torch.randn(B, T, G * cg, generator=g), torch.randn(G * cg, cg, kp, generator=g), torch.randn(G * cg, generator=g)
+    buf = torch.zeros(B, T + 2 * halo, G, cpad, dtype=torch.float64)
+    buf[:, halo:halo + T, :, :cg] = x.double().view(B, T, G, cg)
+    wp = torch.zeros(G * cg, kp, cpad, dtype=torch.float64)
+    wp[:, :, :cg] = w.double().permute(0, 2, 1)
+    rows = B * (T + 2 * halo)
+    buf = torch.cat([buf.view(rows, G, cpad), torch.zeros(kp - 1, G, cpad, dtype=torch.float64)])
+    got = R.grouped_window_ref(buf, wp.view(G * cg, kp * cpad), rows, G, cpad, kp, cg, R.EPI_STORE_F32, bias=b).y
+    want = torch.nn.functional.conv1d(x.double().transpose(1, 2), w.double(), b.double(), padding=halo, groups=G)
+    torch.testing.assert_close(got.view(B, T + 2 * halo, G * cg)[:, :T], want.transpose(1, 2), rtol=1e-12, atol=1e-12)
+    C, T_in = 16, 41
+    T_out = (T_in - 3) // 2 + 1
+    xs, ws = torch.randn(T_in, C, generator=g, dtype=torch.float64), torch.randn(32, C, 3, generator=g, dtype=torch.float64)
+    got = R.gemm_ref(xs.view(-1).as_strided((T_out, 3 * C), (2 * C, 1)), ws.permute(0, 2, 1).reshape(32, 3 * C),
+                     R.EPI_STORE_F32).y
+    want = torch.nn.functional.conv1d(xs.t()[None], ws, stride=2)[0].t()
+    torch.testing.assert_close(got, want, rtol=1e-12, atol=1e-12)
+
+
+@pytest.mark.parametrize("epi,dt", [(R.EPI_STORE_F32, torch.float32), (R.EPI_STORE_BF16, torch.bfloat16)])
+def test_conv_emulation_passes(conv, epi, dt):
+    ref = conv_ref(conv, epi)
+    got = emulate_grouped_conv(conv)
+    r = R.assert_within(got.to(dt), ref.y, ref.mag, R.TAU, dt, extra=ref.extra)
+    print(f"grouped window {dt}: {r:.3g} of the bound")
+    ov = overlap_ref(conv)
+    r = R.assert_within(emulate_overlap(conv), ov.y, ov.mag, R.TAU, torch.float32, extra=ov.extra)
+    print(f"overlapping rows: {r:.3g} of the bound")
+
+
+CONV_MUTATIONS = ["tap_shift", "taps_reversed", "kin_swapped", "group_c0", "b_group_rows", "bias_neighbour", "pitch_K"]
+
+
+@pytest.mark.parametrize("mutation", CONV_MUTATIONS)
+def test_mutated_conv_fails(conv, mutation):
+    """each mistake of the grouped sliding window or the overlapping view lands outside the fp32 bound (run with -s to
+    see by how much)"""
+    if mutation == "pitch_K":
+        ref, got = overlap_ref(conv), emulate_overlap(conv, mutation)
+    else:
+        ref, got = conv_ref(conv), emulate_grouped_conv(conv, mutation)
+    print(f"{mutation}: {_ratio(got, ref.y, R.TAU * ref.mag + ref.extra, torch.float32):.3g} x the bound")
+    with pytest.raises(AssertionError, match="outside the bound"):
+        R.assert_within(got, ref.y, ref.mag, R.TAU, torch.float32, extra=ref.extra)
+
+
+# ----------------------------------------------------------------------------------------------------------------------
 # attention
 # ----------------------------------------------------------------------------------------------------------------------
 AB, AS, AH = 2, 197, 2              # S = 197: three full 64-key blocks and a partial one of 5 keys
