@@ -293,7 +293,8 @@ int opb_infonce_merge_reduce(const float* ws_a, const float* ws_b, int b, int n,
  *   lr, wd, bias_corr          HOST arrays [n_groups <= 128]: lr*lr_scale, weight decay, sqrt(1-b2^t)/(1-b1^t)
  *   grad_scale    device scalar multiplied into every gradient (NULL = 1): out2[1] of opb_grad_norm_clip
  * opb_grad_norm_clip: out2[0] = multiply_factor * ||g||_2, out2[1] = multiply_factor * min(1, max_norm/(norm+1e-6))
- * (max_norm <= 0: no clipping); `partial` is an [n_chunks] fp32 scratch.  Deterministic reduction order.
+ * (max_norm <= 0: no clipping; a NaN norm gives a NaN out2[1]); `partial` is an [n_chunks] fp32 scratch.  Deterministic
+ * reduction order.
  */
 int opb_adam_chunk_elems(void);
 int opb_adam_multi_step(const void* tensors, const int32_t* chunk_tensor, const int64_t* chunk_off, int n_chunks,

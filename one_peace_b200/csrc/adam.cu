@@ -238,7 +238,11 @@ __global__ void grad_norm_finalize_kernel(const float* __restrict__ partial, int
     for (int w = 0; w < (blockDim.x >> 5); ++w) s += red[w];
     const float norm = multiply_factor * static_cast<float>(sqrt(s));
     float coef = 1.f;
-    if (max_norm > 0.f) coef = fminf(1.f, max_norm / (norm + 1e-6f));
+    if (max_norm > 0.f) {
+      // clamp(max=1) that keeps a NaN norm (fminf would drop it): a NaN gradient must poison the step, as in the reference
+      const float r = max_norm / (norm + 1e-6f);
+      coef = r >= 1.f ? 1.f : r;
+    }
     out[0] = norm;
     out[1] = multiply_factor * coef;
   }

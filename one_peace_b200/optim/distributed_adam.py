@@ -21,7 +21,7 @@ import torch
 import torch.distributed as dist
 
 from .. import _lib
-from .adam import _Table
+from .adam import _MAX_GROUPS, _Table
 
 
 def shard_layout(numels, world, align=8):
@@ -80,7 +80,9 @@ class DistributedAdam(torch.optim.Optimizer):
         self.exp_avg_sq = torch.zeros(self.shard, dtype=torch.float32, device=self.device)
         self.segs = shard_segments(self.offsets, numels, self.lo, self.hi)
         self._table, self._norm_table = _Table(), _Table()
-        self.step_count = 0
+        # one step count per parameter, as the reference's python Adam keeps it (optim/adam.py:207-213): a parameter whose
+        # first gradient comes later than its group-mates' gets its own bias correction
+        self.steps = [0] * len(self._plist)
         self._pending = None
         self._has_grad = [True] * len(self._plist)
 
@@ -94,15 +96,16 @@ class DistributedAdam(torch.optim.Optimizer):
 
     def _entries(self):
         """Shard segments of the parameters that received a gradient this step (the reference's python Adam skips
-        `p.grad is None`, adam.py:188-190; every data-parallel rank runs the same graph, so the set is rank-invariant)."""
+        `p.grad is None`, adam.py:188-190; every data-parallel rank runs the same graph, so the set is rank-invariant).
+        The last field is the parameter's (param group, step count) key: the kernel's group table holds one VIRTUAL group per
+        key, as in ``Adam._entries``."""
         out = []
         for pi, _, ln, so in self.segs:
             if not self._has_grad[pi]:
                 continue
-            gi = self._plist[pi][0]
             sl = slice(so, so + ln)
             out.append((self.pshard[sl], self.gshard[sl], self.exp_avg[sl], self.exp_avg_sq[sl],
-                        None if self.master is None else self.master[sl], gi))
+                        None if self.master is None else self.master[sl], (self._plist[pi][0], self.steps[pi] + 1)))
         return out
 
     @torch.no_grad()
@@ -131,7 +134,7 @@ class DistributedAdam(torch.optim.Optimizer):
         sq = torch.zeros(1, dtype=torch.float32, device=self.device)
         if entries:
             nt = self._norm_table
-            nt.build([(e[0], e[1], e[1], e[1], None, e[5]) for e in entries], self.device)
+            nt.build([(e[0], e[1], e[1], e[1], None, 0) for e in entries], self.device)
             out2 = torch.empty(2, dtype=torch.float32, device=self.device)
             st = _lib.load().opb_grad_norm_clip(nt.tensors.data_ptr(), nt.chunk_tensor.data_ptr(), nt.chunk_off.data_ptr(),
                                                 nt.n_chunks, nt.partial.data_ptr(), 1.0, 0.0, out2.data_ptr(),
@@ -176,23 +179,31 @@ class DistributedAdam(torch.optim.Optimizer):
             return loss if loss is not None else norm
         lib = _lib.load()
         stream = torch.cuda.current_stream().cuda_stream
-        # fused Adam on the shard
-        self.step_count += 1
-        t = self._table
-        t.build(entries, self.device)
-        n = len(self.param_groups)
         b1, b2 = self.param_groups[0]["betas"]
         eps = self.param_groups[0]["eps"]
         if any(tuple(g["betas"]) != (b1, b2) or g["eps"] != eps for g in self.param_groups):
             raise NotImplementedError("per-group betas / eps (the reference uses one setting for all groups)")
-        bc = math.sqrt(1 - b2 ** self.step_count) / (1 - b1 ** self.step_count)
-        lr = (ctypes.c_float * n)(*[g["lr"] for g in self.param_groups])
-        wd = (ctypes.c_float * n)(*[g["weight_decay"] for g in self.param_groups])
-        bcs = (ctypes.c_float * n)(*[bc] * n)
+        # virtual groups: one per (param group, step count) in first-seen order
+        vmap = {}
+        for *_, key in entries:
+            vmap.setdefault(key, len(vmap))
+        if len(vmap) > _MAX_GROUPS:
+            raise NotImplementedError("more (param group, step count) combinations than the kernel's group table")
+        keys = list(vmap)
+        n = len(keys)
+        lr = (ctypes.c_float * n)(*[self.param_groups[gi]["lr"] for gi, _ in keys])
+        wd = (ctypes.c_float * n)(*[self.param_groups[gi]["weight_decay"] for gi, _ in keys])
+        bcs = (ctypes.c_float * n)(*[math.sqrt(1 - b2 ** t) / (1 - b1 ** t) for _, t in keys])
+        # fused Adam on the shard
+        t = self._table
+        t.build([e[:5] + (vmap[e[5]],) for e in entries], self.device)
         st = lib.opb_adam_multi_step(t.tensors.data_ptr(), t.chunk_tensor.data_ptr(), t.chunk_off.data_ptr(), t.n_chunks,
                                      ctypes.cast(lr, ctypes.c_void_p), ctypes.cast(wd, ctypes.c_void_p),
                                      ctypes.cast(bcs, ctypes.c_void_p), n, b1, b2, eps, scale.data_ptr(), stream)
-        _lib.check(st, "opb_adam_multi_step")
+        _lib.check(st, "opb_adam_multi_step")       # step counts advance only once the launch was accepted
+        for pi, has in enumerate(self._has_grad):
+            if has:
+                self.steps[pi] += 1
         if self.world > 1:
             dist.all_gather_into_tensor(self.flat_param, self.pshard, group=self.pg)
         else:
@@ -210,7 +221,7 @@ class DistributedAdam(torch.optim.Optimizer):
     def state_dict(self):
         groups = [{k: v for k, v in g.items() if k != "params"} for g in self.param_groups]
         return {"distributed_adam": {"world": self.world, "rank": self.rank, "total": self.total, "shard": self.shard,
-                                     "step": self.step_count, "exp_avg": self.exp_avg.clone(),
+                                     "steps": list(self.steps), "exp_avg": self.exp_avg.clone(),
                                      "exp_avg_sq": self.exp_avg_sq.clone(),
                                      "master": None if self.master is None else self.master.clone()},
                 "param_groups": groups}
@@ -219,7 +230,12 @@ class DistributedAdam(torch.optim.Optimizer):
         st = state_dict["distributed_adam"]
         if (st["world"], st["rank"], st["total"], st["shard"]) != (self.world, self.rank, self.total, self.shard):
             raise ValueError("DistributedAdam state was saved with a different world size / rank / parameter layout")
-        self.step_count = int(st["step"])
+        if "steps" in st:
+            if len(st["steps"]) != len(self.steps):
+                raise ValueError("DistributedAdam state was saved for a different number of parameters")
+            self.steps = [int(t) for t in st["steps"]]
+        else:       # a checkpoint from before per-parameter step counts: one step count for every parameter
+            self.steps = [int(st["step"])] * len(self.steps)
         self.exp_avg.copy_(st["exp_avg"].to(torch.float32))
         self.exp_avg_sq.copy_(st["exp_avg_sq"].to(torch.float32))
         if self.master is not None:

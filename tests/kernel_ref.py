@@ -1,7 +1,8 @@
 """fp64 references of the GEMM epilogues (csrc/gemm_wgmma.cu) and of the convolutions lowered onto that GEMM, of the
 contrastive-head reductions (csrc/infonce.cu), of the attention forward and backward (csrc/attention.cu,
 csrc/attention_bwd.cu) and of the row kernels (csrc/layernorm.cu, csrc/backward.cu, csrc/pack.cu, csrc/gather.cu), with an
-error bound for every output element, and NaN-canary output buffers.
+error bound for every output element, and NaN-canary output buffers; and of the fused Adam step and the gradient norm
+(csrc/adam.cu).
 
 Plain PyTorch on whatever device the inputs live on; nothing here calls the extension.
 
@@ -115,6 +116,42 @@ at 12608 rows, <= 10 + 32 steps in ``partial_reduce_kernel``), so tau = 2^-16 >=
 scatter-adds  (fp32 atomics, ``batch_sum``): onto init, count contributions in any order: (count + 1) u (|init| + sum |g|)
            per destination element.  ``window_scatter`` sums <= kw bf16 terms in a fixed order: kw u sum |terms|, then
            u_out |ref|.
+
+Optimizer (``adam_ref``, ``bf16_param_check``, ``grad_norm_ref``, ``clip_scale_ref``)
+-----------------------------------------------------------------------------------
+csrc/adam.cu, per element in fp32 (``adam_math``):  x = g s;  m' = b1 m + (1 - b1) x;  v' = b2 v + ((1 - b2) x) x;
+d = sqrt(v') + eps;  p1 = p + p (-lr wd) (skipped when lr wd = 0);  p' = p1 + (-lr bc) (m' / d), bc = sqrt(1 - b2^t) /
+(1 - b1^t).  The reference evaluates this in fp64 on the operands the kernel reads (p: the fp32 master, or the bf16
+parameter up-cast; g as stored; m, v; the grad scale s) with the hyperparameters as the user's Python doubles, so the bound
+pays for their fp32 rounding: e_h = |fp32(h) - h| / |h| for h = b1, b2, eps, lr, wd, bc (computed, not assumed), and for
+the kernel's ``1.f - b2``, formed from the already-rounded b2 (exact by Sterbenz for 0.5 <= b < 1):
+e_c2 = |(1 - fp32(b2)) - (1 - b2)| / (1 - b2), 9.5e-7 at b2 = 0.98 and 1.3e-5 at 0.999 (e_c1 likewise).  Bounds are
+absolute, first order, u = 2^-24, every fp32 operation correctly rounded (no fast-math; ``__fdiv_rn``):
+``x``      dx = |g| (u |s| + ds)  (ds: the error of a grad scale that was itself computed, ``clip_scale_ref``)
+``m'``     |b1 m| (e_b1 + u) + (1 - b1) (|x| (e_c1 + u) + dx) + u |m'|
+``v'``     |b2 v| (e_b2 + u) + (1 - b2) (x^2 (e_c2 + 2u) + 2 |x| dx) + u v'      (every term >= 0: no cancellation)
+``sqrt``   sqrt(v') - sqrt(max(v' - dv, 0)) + u sqrt(v'): sqrt is concave, so that fall is larger than the rise
+           sqrt(v' + dv) - sqrt(v'); unlike dv / (2 sqrt v') it stays finite where sqrt(v') ~ 0 (|g| ~ eps)
+``d``      d_sqrt + eps e_eps + u d
+``q``      q = m' / d: dm / d + |q| dd / d + u |q|
+``upd``    lr bc q: lr bc dq + |upd| (e_lr + e_bc + 2u)                (step_size = fp32(lr) fp32(bc) rounded, the product)
+``p1``     |p lr wd| (e_lr + e_wd + 2u) + u |p1|
+``p'``     dp1 + dupd + u |p'|
+bf16 parameters: with a master copy the kernel stores bf16_rn(master') from the same register, so p16 == bf16_rn(master')
+bit for bit.  Without one, p16 is bf16_rn of the fp32 p', which lies within dp' of the fp64 p'; rounding is monotone, so
+p16 must lie between bf16_rn(p' - dp') and bf16_rn(p' + dp'): equal to bf16_rn(p') except where p' is within dp' of a
+rounding midpoint, where either neighbour passes.
+
+Gradient norm: ``grad_sumsq_kernel`` runs grid = min(n_chunks, 1056) CTAs of 256 threads; CTA b owns chunks b, b + grid,
+...  Each thread adds its <= 32 elements of each chunk (8 float4 or 4 x 8 bf16 vector loads of a full aligned chunk,
+else a 256-strided scalar loop) into one fp32 register, squares rounded once (or fused), then 5 shuffle levels and a
+serial sum of the 8 warp partials.  Every term is >= 0, so the fp32 sum of squares is off by at most
+depth u S, depth = 1 + 32 ceil(n_chunks / grid) + 5 + 8.  The finalize kernel sums the grid partials in fp64 (1024 threads
+strided, 5 shuffle levels, 32 warp partials: <= 40 additions, 2^-53 each), sqrt in fp64, rounds to fp32 (u) and
+multiplies by fp32(multiply_factor) (u + e_mf): rel(norm) = depth u / 2 + 41 * 2^-53 + 2u + e_mf.  The clip coefficient
+min(1, max_norm / (norm + 1e-6)) is off by r (dnorm / (norm + 1e-6) + |fp32(1e-6) - 1e-6| / (norm + 1e-6) + e_max_norm +
+k u), k = 2 fp32 roundings in the kernel (the sum, the division); min(1, .) does not increase it.  grad_scale =
+multiply_factor coef: |mf| dcoef + |grad_scale| (e_mf + u).
 """
 from types import SimpleNamespace
 
@@ -747,3 +784,114 @@ def window_scatter_ref(dwin, B, t_in, t_out, stride, kw, pad):
                 out[:, s] += v
                 mag[:, s] += v.abs()
     return out.reshape(B * t_in, groups * cg), kw * U32 * mag.reshape(B * t_in, groups * cg)
+
+
+# ----------------------------------------------------------------------------------------------------------------------
+# optimizer (module docstring, "Optimizer")
+# ----------------------------------------------------------------------------------------------------------------------
+ADAM_CHUNK = 8192               # opb_adam_chunk_elems()
+NORM_GRID_CAP = 132 * 8         # grad_sumsq_kernel: grid = min(n_chunks, 1056)
+U64 = 2.0 ** -53
+
+
+def f32_rel(x):
+    """relative error of rounding the Python double x to fp32 (0 for x = 0)"""
+    x = float(x)
+    return 0.0 if x == 0 else abs(float(np.float32(x)) - x) / abs(x)
+
+
+def bias_correction(t, betas):
+    """sqrt(1 - b2^t) / (1 - b1^t) in Python doubles, as the optimizers pass it to the kernel"""
+    b1, b2 = betas
+    return (1 - b2 ** t) ** 0.5 / (1 - b1 ** t)
+
+
+def adam_ref(p, g, m, v, *, t, lr, wd, betas, eps, grad_scale=None, grad_scale_err=0.0):
+    """fp64 Adam step of ``adam_math`` on the operands the kernel reads (p: fp32 master or bf16 parameter; g fp32 or bf16;
+    m, v fp32), t the step count after this step, lr including lr_scale, grad_scale a Python float (None = 1) with the
+    absolute error ``grad_scale_err`` of its computed value.  Returns a namespace with m, m_err, v, v_err, p, p_err (the fp32
+    p' of the master copy or an fp32 parameter) and upd, upd_err (lr bc m' / d)."""
+    b1, b2 = betas
+    assert 0.5 <= b1 < 1 and 0.5 <= b2 < 1, "1 - fp32(b) is exact only for 0.5 <= b < 1"
+    u = U32
+    P, G, M0, V0 = (x.double() for x in (p, g, m, v))
+    s = 1.0 if grad_scale is None else float(grad_scale)
+    c1, c2 = 1 - b1, 1 - b2
+    e_c1 = abs((1 - float(np.float32(b1))) - c1) / c1
+    e_c2 = abs((1 - float(np.float32(b2))) - c2) / c2
+    X = G * s
+    dX = G.abs() * (u * abs(s) + grad_scale_err)
+    Mn = b1 * M0 + c1 * X
+    dM = (b1 * M0).abs() * (f32_rel(b1) + u) + c1 * (X.abs() * (e_c1 + u) + dX) + u * Mn.abs()
+    Vn = b2 * V0 + c2 * X * X
+    dV = (b2 * V0).abs() * (f32_rel(b2) + u) + c2 * (X * X * (e_c2 + 2 * u) + 2 * X.abs() * dX) + u * Vn.abs()
+    R = Vn.sqrt()
+    dR = R - (Vn - dV).clamp_min(0.0).sqrt() + u * R
+    D = R + eps
+    dD = dR + eps * f32_rel(eps) + u * D
+    Q = Mn / D
+    dQ = dM / D + Q.abs() * dD / D + u * Q.abs()
+    bc = bias_correction(t, betas)
+    Upd = lr * bc * Q
+    dUpd = lr * bc * dQ + Upd.abs() * (f32_rel(lr) + f32_rel(bc) + 2 * u)
+    if float(np.float32(wd)) * float(np.float32(lr)) != 0.0:
+        P1 = P * (1 - lr * wd)
+        dP1 = (P * lr * wd).abs() * (f32_rel(lr) + f32_rel(wd) + 2 * u) + u * P1.abs()
+    else:
+        P1, dP1 = P, torch.zeros_like(P)
+    Pn = P1 - Upd
+    dPn = dP1 + dUpd + u * Pn.abs()
+    return SimpleNamespace(m=Mn, m_err=dM, v=Vn, v_err=dV, p=Pn, p_err=dPn, upd=Upd, upd_err=dUpd)
+
+
+def bf16_param_check(got, ref, err, what="bf16 parameter"):
+    """bf16 parameter written without a master copy: bf16_rn of some fp32 value within ``err`` of ``ref``, i.e. between
+    bf16_rn(ref - err) and bf16_rn(ref + err) (rounding is monotone).  Returns the number of elements where both
+    neighbours were allowed (ref within err of a rounding midpoint)."""
+    lo = (ref - err).bfloat16().double()
+    hi = (ref + err).bfloat16().double()
+    g = got.double()
+    bad = ~((g >= lo) & (g <= hi))
+    n_bad = int(bad.sum().item())
+    if n_bad:
+        i = int(bad.flatten().nonzero()[0].item())
+        raise AssertionError(f"{what}: {n_bad} of {g.numel()} elements outside the bound; first at {i}: got "
+                             f"{g.flatten()[i].item()!r}, allowed [{lo.flatten()[i].item()!r}, {hi.flatten()[i].item()!r}] "
+                             f"(ref {ref.flatten()[i].item()!r} +- {err.flatten()[i].item():.3e})")
+    return int((lo != hi).sum().item())
+
+
+def norm_chunks(numels, chunk=ADAM_CHUNK):
+    """the chunk table of ``optim.adam._Table``: [(tensor index, element offset, length)] in table order"""
+    return [(i, o, min(chunk, n - o)) for i, n in enumerate(numels) for o in range(0, n, chunk)]
+
+
+def clip_scale_ref(norm, norm_err, multiply_factor, max_norm, roundings=2):
+    """grad_scale = multiply_factor * min(1, max_norm / (norm + 1e-6)) (multiply_factor alone for max_norm <= 0) from an fp64
+    norm with absolute error ``norm_err``; ``roundings``: fp32 roundings between the norm and the coefficient (2 in the
+    kernel: the sum and the division).  -> (grad_scale, bound)"""
+    mf = float(multiply_factor)
+    if max_norm <= 0:
+        return mf, abs(mf) * f32_rel(mf)
+    den = norm + 1e-6
+    r = max_norm / den
+    dr = r * ((norm_err + abs(float(np.float32(1e-6)) - 1e-6)) / den + f32_rel(max_norm) + roundings * U32)
+    gs = mf * (1.0 if r >= 1.0 else r)          # clamp(max=1), keeping a NaN
+    return gs, abs(mf) * dr + abs(gs) * (f32_rel(mf) + U32)
+
+
+def grad_norm_ref(grads, multiply_factor=1.0, max_norm=0.0, chunk=ADAM_CHUNK):
+    """fp64 ``opb_grad_norm_clip`` over the gradients in table order (module docstring, "Optimizer").  Returns a namespace
+    with n_chunks, grid, depth (of the fp32 sum of squares), sumsq, norm (multiply_factor ||g||_2), norm_err, scale
+    (out[1]) and scale_err."""
+    n_chunks = len(norm_chunks([x.numel() for x in grads], chunk))
+    grid = min(n_chunks, NORM_GRID_CAP)
+    depth = 1 + 32 * -(-n_chunks // grid) + 5 + 8
+    S = sum(float(x.double().square().sum()) for x in grads)
+    raw = S ** 0.5
+    mf = float(multiply_factor)
+    N = mf * raw
+    dN = abs(N) * (depth * U32 / 2 + 41 * U64 + 2 * U32 + f32_rel(mf))
+    gs, dgs = clip_scale_ref(N, dN, mf, max_norm)
+    return SimpleNamespace(n_chunks=n_chunks, grid=grid, depth=depth, sumsq=S, norm=N, norm_err=dN, scale=gs,
+                           scale_err=dgs)

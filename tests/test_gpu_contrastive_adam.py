@@ -119,49 +119,6 @@ def test_adam_vs_reference_golden(golden_dir, tag):
     torch.testing.assert_close(st["exp_avg_sq"].cpu(), fx["exp_avg_sq"], atol=1e-10, rtol=2e-6)
 
 
-def test_adam_multi_tensor_groups_clip_and_master():
-    """Many tensors (odd sizes, two groups with lr_scale / no-decay as utils/layer_decay.py builds them), grad-norm
-    clipping folded into the step, fp32 master weights; oracle = restated.adam_step + clip_coefficient."""
-    need_gpu()
-    from one_peace_b200.optim import Adam, MemoryEfficientBF16Optimizer, AdjustAdam
-    g = torch.Generator().manual_seed(0)
-    shapes = [(1536, 384), (1536,), (77,), (3, 5, 7), (8193,), (1,), (50000,)]
-    ps = [torch.randn(s, generator=g) for s in shapes]
-    gs = [[torch.randn(s, generator=g) * 0.3 for s in shapes] for _ in range(2)]
-
-    class Cfg:
-        lr = [1e-2]; adam_betas = "(0.9, 0.98)"; adam_eps = 1e-8; weight_decay = 0.05; master_weights = True
-    params = [torch.nn.Parameter(p.clone().bfloat16().cuda()) for p in ps]
-    groups = [dict(params=params[:3], weight_decay=0.05, lr_scale=0.5), dict(params=params[3:], weight_decay=0.0, lr_scale=1.0)]
-    fo = AdjustAdam(Cfg, groups)
-    fo.set_lr(1e-2)
-    opt = MemoryEfficientBF16Optimizer(fo)
-    # oracle state (fp32 master, python form)
-    om = [p.bfloat16().float() for p in ps]
-    m = [torch.zeros_like(p) for p in ps]; v = [torch.zeros_like(p) for p in ps]
-    for step, grads in enumerate(gs, start=1):
-        for p, gr in zip(params, grads):
-            p.grad = gr.bfloat16().cuda()
-        opt.multiply_grads(0.5)
-        norm = opt.clip_grad_norm(1.0)
-        opt.step()
-        gb = [gr.bfloat16().float() for gr in grads]
-        wnorm, coef = R.clip_coefficient(gb, 1.0, multiply_factor=0.5)
-        assert abs(norm.item() - wnorm) / wnorm < 1e-5
-        for i in range(len(ps)):
-            lr = 1e-2 * (0.5 if i < 3 else 1.0)
-            wd = 0.05 if i < 3 else 0.0
-            R.adam_step(om[i], gb[i] * (0.5 * coef), m[i], v[i], step, lr, 0.9, 0.98, 1e-8, wd)
-    for i, p in enumerate(params):
-        master = opt.optimizer.state[p]["master"].cpu()
-        torch.testing.assert_close(master, om[i], atol=2e-6, rtol=2e-5)
-        assert torch.equal(p.detach().cpu(), master.bfloat16())
-    # determinism of the norm: same grads -> bit-identical norm
-    n1 = opt.optimizer.grad_norm_and_scale(1.0, 0.0)[0].item()
-    n2 = opt.optimizer.grad_norm_and_scale(1.0, 0.0)[0].item()
-    assert n1 == n2
-
-
 def test_two_rank_contrastive_step_nccl():
     """configs[3] at W = 2 on real GPUs: NCCL all-gather + InfoNCE fwd/bwd vs the oracle (skipped on a 1-GPU box;
     it needs two GPUs)."""
@@ -264,30 +221,3 @@ def test_adam_state_survives_load_state_dict_with_bf16_params():
         oa.step(); ob.step()
     for p, q in zip(pa, pb):
         assert torch.equal(p.detach(), q.detach()) and torch.equal(oa.state[p]["master"], ob.state[q]["master"])
-
-
-def test_adam_per_parameter_step_counts():
-    """ADVICE r1 (low): a parameter that gets its first gradient later than its group-mates keeps its own bias correction
-    (optim/adam.py:207-213 tracks `step` per parameter)."""
-    need_gpu()
-    from one_peace_b200.optim import Adam
-    g = torch.Generator().manual_seed(4)
-    a0, b0 = torch.randn(300, generator=g), torch.randn(200, generator=g)
-    ga = [torch.randn(300, generator=g) for _ in range(3)]
-    gb = [None, torch.randn(200, generator=g), torch.randn(200, generator=g)]
-    pa, pb = torch.nn.Parameter(a0.clone().cuda()), torch.nn.Parameter(b0.clone().cuda())
-    opt = Adam([pa, pb], lr=1e-2, betas=(0.9, 0.98), eps=1e-8, weight_decay=0.05)
-    wa, wb = a0.clone(), b0.clone()
-    ma, va, mb, vb = torch.zeros(300), torch.zeros(300), torch.zeros(200), torch.zeros(200)
-    tb = 0
-    for t in range(3):
-        pa.grad = ga[t].cuda()
-        pb.grad = None if gb[t] is None else gb[t].cuda()
-        opt.step()
-        R.adam_step(wa, ga[t], ma, va, t + 1, 1e-2, 0.9, 0.98, 1e-8, 0.05)
-        if gb[t] is not None:
-            tb += 1
-            R.adam_step(wb, gb[t], mb, vb, tb, 1e-2, 0.9, 0.98, 1e-8, 0.05)
-    torch.testing.assert_close(pa.detach().cpu(), wa, atol=1e-6, rtol=1e-5)
-    torch.testing.assert_close(pb.detach().cpu(), wb, atol=1e-6, rtol=1e-5)
-    assert opt.state[pa]["step"] == 3 and opt.state[pb]["step"] == 2

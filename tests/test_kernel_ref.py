@@ -767,3 +767,240 @@ def test_row_mutation_fails(rowk, sres, mutation):
     name = max(ratios, key=ratios.get)
     print(f"{mutation}: {name} exceeds its bound {ratios[name]:.3g}-fold")
     assert ratios[name] >= 10, ratios
+
+
+# ----------------------------------------------------------------------------------------------------------------------
+# optimizer
+# ----------------------------------------------------------------------------------------------------------------------
+OPT_BETAS, OPT_EPS, OPT_GS = (0.9, 0.98), 1e-8, 0.37
+# (lr, wd) per param group: lr = 1e-2 with wd = 0.05 puts the order of decay and update above u |p|; a layer-decayed
+# group (lr_scale 0.5) and a no-decay group
+OPT_GROUPS = [(1e-2, 0.05), (0.5 * 1e-3, 0.05), (1e-3, 0.0)]
+# (param group, step count t after the step, parameter kind): "f32", "bf16" (no master copy), "master" (bf16 + fp32 master)
+OPT_TENSORS = [(0, 1, "f32"), (1, 2, "bf16"), (2, 10, "master"), (0, 1000, "f32"), (0, 2, "bf16"), (1, 10, "f32"),
+               (2, 1, "bf16"), (0, 10, "master")]
+OPT_N = 4096
+
+
+def _opt_state(t, n, band, g):
+    """m, v as a step count of t - 1 leaves them: zero at t = 1, else moments of gradients of the same scale"""
+    if t == 1:
+        return torch.zeros(n), torch.zeros(n)
+    b1, b2 = OPT_BETAS
+    scale = torch.where(band, 1e-7, 0.3)
+    h1, h2 = torch.randn(n, generator=g) * scale, torch.randn(n, generator=g) * scale
+    return (1 - b1 ** (t - 1)) * h1, (1 - b2 ** (t - 1)) * h2 * h2
+
+
+@pytest.fixture(scope="module")
+def opt():
+    """every 4th gradient in a band 1e-9 <= |g| <= 1e-6 (sqrt(v) comparable to eps), every 16th gradient and state zero"""
+    g = torch.Generator().manual_seed(11)
+    tensors = []
+    for gi, t, kind in OPT_TENSORS:
+        i = torch.arange(OPT_N)
+        band = i % 4 == 1
+        grad = torch.randn(OPT_N, generator=g) * 0.3
+        grad[band] = torch.sign(grad[band]) * 10.0 ** (-9 + 3 * torch.rand(int(band.sum()), generator=g))
+        m, v = _opt_state(t, OPT_N, band, g)
+        zero = i % 16 == 3
+        grad[zero], m[zero], v[zero] = 0.0, 0.0, 0.0
+        p = torch.randn(OPT_N, generator=g)
+        if kind != "f32":
+            p = p.bfloat16().float()
+        tensors.append(dict(group=gi, t=t, kind=kind, p=p, g=grad, m=m, v=v))
+    vgroups = list(dict.fromkeys((T["group"], T["t"]) for T in tensors))
+    return dict(tensors=tensors, vgroups=vgroups)
+
+
+def _bits_trunc_bf16(x):
+    """bf16 by truncation (the mistake): drop the low 16 bits of the fp32 pattern"""
+    return (x.view(torch.int32) & -65536).view(torch.float32).bfloat16()
+
+
+def emulate_adam(d, mutation=None):
+    """fp32 emulation of adam_multi_kernel in ``adam_math``'s order of operations, optionally with one planted mistake.
+    -> per tensor (m', v', fp32 p' (None for bf16 without a master copy), bf16 p' (None for fp32))"""
+    f = lambda x: torch.tensor(float(x), dtype=torch.float32)
+    b1, b2 = OPT_BETAS[::-1] if mutation == "betas_swapped" else OPT_BETAS
+    b1f, b2f, epsf, gs = f(b1), f(b2), f(OPT_EPS), f(OPT_GS)
+    out = []
+    for T in d["tensors"]:
+        lr, wd = OPT_GROUPS[T["group"]]
+        t = T["t"]
+        vg = d["vgroups"].index((T["group"], t))
+        if mutation == "bias_corr_t_minus_1" and t > 1:          # (at t = 1 the lagging count gives 0 / 0)
+            t = t - 1
+        if mutation == "bias_corr_neighbour_group":
+            t = d["vgroups"][(vg + 1) % len(d["vgroups"])][1]
+        bc = R.bias_correction(t, OPT_BETAS)
+        p, m, v = T["p"].clone(), T["m"].clone(), T["v"].clone()
+        x = T["g"] * gs
+        lr_wd = f(wd) * f(lr)
+        if mutation == "wd_into_g":
+            x = x + f(wd) * p
+        m = m * b1f + x * (1 - b1f)
+        xv = T["g"] if mutation == "grad_scale_m_only" else x
+        v = v * b2f + ((1 - b2f) * xv) * xv
+        step = f(lr) * f(bc)
+        if mutation == "eps_after_bias_correction":          # torch AdamW: lr m_hat / (sqrt(v_hat) + eps)
+            q = (m / f(1 - b1 ** t)) / (torch.sqrt(v / f(1 - b2 ** t)) + epsf)
+            step = f(lr)
+        else:
+            q = m / (torch.sqrt(v) + epsf)
+        decay = lr_wd != 0 and mutation != "wd_into_g"
+        if decay and mutation != "wd_after_update":
+            p = p + p * -lr_wd
+        p = p + -step * q
+        if decay and mutation == "wd_after_update":
+            p = p + p * -lr_wd
+        p16 = None if T["kind"] == "f32" else (_bits_trunc_bf16(p) if mutation == "bf16_truncated" else p.bfloat16())
+        out.append((m, v, None if T["kind"] == "bf16" else p, p16))
+    return out
+
+
+def adam_outputs(d, mutation=None):
+    """{name: (got, ref, bound)} for every output of every tensor; a bf16 parameter without a master copy appears as its
+    distance outside the allowed interval [bf16_rn(p' - dp'), bf16_rn(p' + dp')] against a bound of dp'"""
+    res = {}
+    for k, (T, (m, v, p32, p16)) in enumerate(zip(d["tensors"], emulate_adam(d, mutation))):
+        lr, wd = OPT_GROUPS[T["group"]]
+        r = R.adam_ref(T["p"], T["g"], T["m"], T["v"], t=T["t"], lr=lr, wd=wd, betas=OPT_BETAS, eps=OPT_EPS,
+                       grad_scale=OPT_GS)
+        res[f"t{k} m"] = (m, r.m, r.m_err)
+        res[f"t{k} v"] = (v, r.v, r.v_err)
+        if p32 is not None:
+            res[f"t{k} p"] = (p32, r.p, r.p_err)
+        if T["kind"] == "master":
+            res[f"t{k} p16 == bf16(master)"] = (p16.double(), p32.bfloat16().double(), torch.zeros(OPT_N, dtype=torch.float64))
+        if T["kind"] == "bf16":
+            lo, hi = (r.p - r.p_err).bfloat16().double(), (r.p + r.p_err).bfloat16().double()
+            gd = p16.double()
+            res[f"t{k} p16"] = ((gd - hi).clamp_min(0) + (lo - gd).clamp_min(0), torch.zeros_like(gd), r.p_err)
+    return res
+
+
+def test_adam_reference_is_python_adam(opt):
+    """adam_ref in fp64 is oracle/restated.adam_step (the reference's python Adam) run in fp64"""
+    import restated
+    for T in opt["tensors"]:
+        lr, wd = OPT_GROUPS[T["group"]]
+        r = R.adam_ref(T["p"], T["g"], T["m"], T["v"], t=T["t"], lr=lr, wd=wd, betas=OPT_BETAS, eps=OPT_EPS,
+                       grad_scale=OPT_GS)
+        p, m, v = T["p"].double(), T["m"].double(), T["v"].double()
+        restated.adam_step(p, T["g"].double() * OPT_GS, m, v, T["t"], lr, *OPT_BETAS, OPT_EPS, wd)
+        for got, want in ((p, r.p), (m, r.m), (v, r.v)):
+            torch.testing.assert_close(got, want, rtol=1e-12, atol=1e-15)
+
+
+def test_adam_emulation_passes(opt):
+    for name, (got, ref, bound) in adam_outputs(opt).items():
+        r = R.assert_within(got, ref, bound, 1.0, torch.float32, what=name)
+        print(f"adam {name}: {r:.3g} of the bound")
+    for T, (_, _, _, p16) in zip(opt["tensors"], emulate_adam(opt)):
+        if T["kind"] == "bf16":
+            lr, wd = OPT_GROUPS[T["group"]]
+            r = R.adam_ref(T["p"], T["g"], T["m"], T["v"], t=T["t"], lr=lr, wd=wd, betas=OPT_BETAS, eps=OPT_EPS,
+                           grad_scale=OPT_GS)
+            amb = R.bf16_param_check(p16, r.p, r.p_err)
+            assert amb < OPT_N // 100, amb       # the either-neighbour band is a few elements, not a percentage
+
+
+ADAM_MUTATIONS = ["bias_corr_t_minus_1", "bias_corr_neighbour_group", "eps_after_bias_correction", "wd_after_update",
+                  "wd_into_g", "grad_scale_m_only", "betas_swapped", "bf16_truncated"]
+
+
+@pytest.mark.parametrize("mutation", ADAM_MUTATIONS)
+def test_adam_mutation_fails(opt, mutation):
+    """each mistake exceeds the bound at least ten-fold on at least one output (run with -s to see the factors)"""
+    outs = adam_outputs(opt, mutation)
+    ratios = {name: _ratio(got, ref, bound, torch.float32) for name, (got, ref, bound) in outs.items()}
+    name = max(ratios, key=ratios.get)
+    assert ratios[name] >= 10, ratios
+    # the factor printed leaves out elements whose bound is 0 (exact results, e.g. zero state), where any error is infinite
+    finite = {n: _ratio(got[bound > 0], ref[bound > 0], bound[bound > 0], torch.float32)
+              for n, (got, ref, bound) in outs.items() if (bound > 0).any()}
+    name = max(finite, key=finite.get)
+    print(f"{mutation}: {name} exceeds its bound {finite[name]:.3g}-fold")
+
+
+# gradient norm: 1100 tiny tensors, then a two-chunk tensor with a 1000-element tail chunk and a bf16-valued one, so that
+# 1105 chunks > 1056 CTAs and the last CTAs' second chunks are the big ones
+@pytest.fixture(scope="module")
+def norm_grads():
+    g = torch.Generator().manual_seed(12)
+    sizes = (torch.randint(1, 200, (1100,), generator=g)).tolist() + [2 * R.ADAM_CHUNK + 1000, R.ADAM_CHUNK + 5]
+    grads = [torch.randn(n, generator=g) * (0.1 + torch.rand(1, generator=g)) for n in sizes]
+    grads[-1] = grads[-1].bfloat16().float()
+    return grads
+
+
+def emulate_grad_norm(grads, mf, max_norm, mutation=None):
+    """fp32 emulation of grad_sumsq_kernel (per-thread order, shuffle tree, warp partials) and grad_norm_finalize_kernel"""
+    chunks = R.norm_chunks([x.numel() for x in grads])
+    grid = min(len(chunks), R.NORM_GRID_CAP)
+    acc = torch.zeros(grid, 256)
+    for c, (ti, off, n) in enumerate(chunks):
+        if mutation == "second_chunk_dropped" and c >= grid:
+            continue
+        if mutation == "tail_chunk_dropped" and n < R.ADAM_CHUNK and grads[ti].numel() > R.ADAM_CHUNK:
+            continue
+        x = grads[ti][off:off + n]
+        if n == R.ADAM_CHUNK:            # vector path: per thread 8 loads of 4 elements, ((a + b) + c) + d added per load
+            sq = (x * x).view(8, 256, 4)
+            terms = torch.zeros(256, 32)
+            terms[:, ::4] = (((sq[..., 0] + sq[..., 1]) + sq[..., 2]) + sq[..., 3]).t()
+        else:                            # scalar path: thread t adds elements t, t + 256, ...
+            terms = torch.nn.functional.pad(x * x, (0, R.ADAM_CHUNK - n)).view(32, 256).t()
+        b = c % grid
+        for j in range(32):
+            acc[b] = acc[b] + terms[:, j]
+    w = acc.view(grid, 8, 32)
+    for o in (16, 8, 4, 2, 1):
+        w = w + w[:, :, torch.arange(32) ^ o]
+    part = torch.zeros(grid)
+    for k in range(8):
+        part = part + w[:, k, 0]
+    s = float(part.double().sum())
+    mff = torch.tensor(1.0 if mutation == "no_multiply_factor" else mf, dtype=torch.float32)
+    norm = mff * torch.tensor(s ** 0.5, dtype=torch.float32)
+    r = torch.tensor(max_norm, dtype=torch.float32) / (norm + torch.tensor(1e-6, dtype=torch.float32))
+    coef = torch.where(r >= 1, torch.ones(()), r) if max_norm > 0 else torch.ones(())
+    return norm, torch.tensor(mf, dtype=torch.float32) * coef
+
+
+NORM_MUTATIONS = ["second_chunk_dropped", "tail_chunk_dropped", "no_multiply_factor"]
+
+
+def norm_outputs(grads, mutation=None):
+    mf = 0.37
+    ref0 = R.grad_norm_ref(grads, mf)
+    ref = R.grad_norm_ref(grads, mf, 0.5 * ref0.norm)          # clips to half
+    norm, scale = emulate_grad_norm(grads, mf, 0.5 * ref0.norm, mutation)
+    d = lambda x: torch.tensor([x], dtype=torch.float64)
+    return ref, {"norm": (norm.reshape(1), d(ref.norm), d(ref.norm_err)), "scale": (scale.reshape(1), d(ref.scale), d(ref.scale_err))}
+
+
+def test_grad_norm_emulation_passes(norm_grads):
+    ref, outs = norm_outputs(norm_grads)
+    assert ref.n_chunks == 1105 and ref.grid == 1056 and ref.depth == 1 + 64 + 13
+    for name, (got, want, bound) in outs.items():
+        r = R.assert_within(got, want, bound, 1.0, torch.float32, what=name)
+        print(f"grad norm {name}: {r:.3g} of the bound")
+
+
+@pytest.mark.parametrize("mutation", NORM_MUTATIONS)
+def test_grad_norm_mutation_fails(norm_grads, mutation):
+    _, outs = norm_outputs(norm_grads, mutation)
+    ratios = {name: _ratio(got, want, bound, torch.float32) for name, (got, want, bound) in outs.items()}
+    name = max(ratios, key=ratios.get)
+    print(f"{mutation}: {name} exceeds its bound {ratios[name]:.3g}-fold")
+    assert ratios[name] >= 10, ratios
+
+
+def test_clip_scale_keeps_nan_and_zeroes_inf():
+    """the reference of out[1]: a NaN norm gives a NaN scale (clamp(max=1) keeps it), an infinite one a zero scale"""
+    import math
+    assert math.isnan(R.clip_scale_ref(float("nan"), 0.0, 1.0, 1.0)[0])
+    assert R.clip_scale_ref(float("inf"), 0.0, 0.5, 1.0)[0] == 0.0
+    assert R.clip_scale_ref(3.0, 0.0, 0.5, 0.0) == (0.5, 0.0)
