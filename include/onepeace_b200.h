@@ -488,6 +488,32 @@ int opb_classify_loss(const float* logits, int64_t ld, int rows, int n_valid, in
                       const float* targets, int64_t ld_t, float eps, int num_choices, float* row_loss, float* dlogits,
                       float* row_correct, float* out2, unsigned int* ticket, void* stream);
 
+/* ------------------------------------------------------------------------------------------------------------------
+ * Visual grounding (refcoco_criterion and IouAcc).
+ *   opb_refcoco_loss : criterions/refcoco_loss.py:36-46 and its gradient with respect to the logits, in fp32, in one launch.
+ *                      p = sigmoid(logits[r, 0:4]) against targets fp32 [B, 4] (x0, y0, x1, y1, contiguous):
+ *                        L1 = sum_{r,j} |p - t| / nsentences, gradient sign(p - t) / nsentences (0 at a tie);
+ *                        valid[r] = p0 < p2 && p1 < p3 (strict; selects rows, no gradient through it);
+ *                        giou[r] = torchvision.ops.generalized_box_iou of (p_r, t_r), written for every row;
+ *                        loss = L1 + sum over valid rows of (1 - giou) / n_valid; NaN when n_valid == 0 (the reference's
+ *                        mean of an empty tensor), while the gradient stays finite: the L1 part only.
+ *                      The GIoU gradient follows torch's autograd: max / min give half the gradient to each side at a tie,
+ *                      clamp(min=0) passes it where its argument is >= 0, and the targets get none.
+ *                      logits fp32 [B, ld], ld >= 4 (columns [4, ld) are not read); out fp32 [3] = {loss, L1 part, n_valid};
+ *                      valid int32 [B]; giou fp32 [B]; dlogits fp32 [B, ld] = d loss / d logits with columns [4, ld) set to
+ *                      0.  One CTA, fixed-order sums: repeated launches are bit-identical.  Status 1 for B <= 0, ld < 4,
+ *                      nsentences <= 0 or a null pointer, before anything is launched.
+ *   opb_iou_acc      : metrics/iou_acc.py:20-32: hits[0] += number of rows r < n with iou >= 0.5 and w_i > 0 and h_i > 0, where
+ *                      the intersection takes the max / min corners and iou = area_i / (area_p + area_t - area_i), every
+ *                      operation in the reference's order and rounded on its own (no FMA contraction), so the count equals
+ *                      the reference's fp32 count exactly.  hyps / refs fp32 [n, >= 4] at row pitches ld_h / ld_r; hits one
+ *                      int32 the caller zeroes once and reads when it wants the total (nothing synchronises); row_hit int32
+ *                      [n] or NULL receives the per-row flag.  Status 1 for n <= 0, a pitch < 4 or a null hyps / refs / hits.
+ * ------------------------------------------------------------------------------------------------------------------ */
+int opb_refcoco_loss(const float* logits, int64_t ld, const float* targets, int B, int nsentences, float* out, int* valid,
+                     float* giou, float* dlogits, void* stream);
+int opb_iou_acc(const float* hyps, int64_t ld_h, const float* refs, int64_t ld_r, int n, int* hits, int* row_hit, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

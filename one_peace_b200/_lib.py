@@ -103,6 +103,8 @@ SIGNATURES.update({
                                   c_int, c_void_p]),
     "opb_classify_loss": (c_int, [c_void_p, c_int64, c_int, c_int, c_int, c_void_p, c_void_p, c_int64, c_float, c_int, c_void_p,
                                   c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "opb_refcoco_loss": (c_int, [c_void_p, c_int64, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "opb_iou_acc": (c_int, [c_void_p, c_int64, c_void_p, c_int64, c_int, c_void_p, c_void_p, c_void_p]),
 })
 
 

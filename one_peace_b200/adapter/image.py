@@ -31,6 +31,35 @@ def make_image_bucket_position(bucket_size, num_relative_distance):
     return idx
 
 
+def geometric_sequence_interpolation(src_size, dst_size, sequence, num):
+    """models/adapter/image.py:115-162: resample a (src_size x src_size) relative-position table [src_size^2, num] onto
+    (dst_size x dst_size).  The source offsets are placed on a geometric sequence whose ratio q (bisection over [1.01, 1.5]
+    down to 1e-6) stretches src_size // 2 steps to dst_size // 2, and every head is fitted by a bicubic interpolating spline
+    evaluated on the integer offsets -t .. t.  The reference calls scipy.interpolate.interp2d(kind='cubic'), which SciPy 1.14
+    removed; on gridded data it computed the s = 0 bicubic spline of RectBivariateSpline(y, x, z), which is what runs here
+    (z is [len(y), len(x)])."""
+    import numpy as np
+    from scipy.interpolate import RectBivariateSpline
+
+    half_src, half_dst = src_size // 2, dst_size // 2
+    lo, hi = 1.01, 1.5
+    while hi - lo > 1e-6:                      # sum_{k<half_src} q^k against half_dst
+        q = (lo + hi) / 2.0
+        lo, hi = (lo, q) if (1.0 - q ** half_src) / (1.0 - q) > half_dst else (q, hi)
+    pos = [1]
+    for k in range(1, half_src):
+        pos.append(pos[-1] + q ** k)
+    grid = np.array([-v for v in pos[::-1]] + [0] + pos, dtype=np.float64)
+    t = dst_size // 2.0
+    target = np.arange(-t, t + 0.1, 1.0)
+    heads = []
+    for h in range(num):
+        z = sequence[:, h].view(src_size, src_size).float().numpy()
+        spline = RectBivariateSpline(grid, grid, z, kx=3, ky=3, s=0)       # axis 0 = y (rows of z), axis 1 = x
+        heads.append(torch.tensor(spline(target, target), dtype=torch.float32).reshape(-1, 1).to(sequence))
+    return torch.cat(heads, dim=-1)
+
+
 class LayerNorm2D(torch.nn.Module):
     """Parameter container named like models/adapter/image.py:37-47 (embed_images.{1,4}.layer_norm.*)."""
 
@@ -182,6 +211,31 @@ class ImageAdapter(torch.nn.Module):
         K.cls_row_init(p["cls"], pos, x)
         bias = self.get_rel_pos_bias(S) if self.rel_pos_table_list is not None else None
         return x, None, bias
+
+    def upgrade_state_dict_named(self, state_dict, name):
+        """Resize a checkpoint's image tables to this adapter (models/adapter/image.py:262-305): a relative-position table
+        smaller than (2 * rel_bucket_size - 1)^2 + 3 rows (a 256^2 checkpoint loaded for 384^2 fine-tuning) is interpolated
+        onto the larger grid, and pos_embed is resized bicubically when it has fewer than bucket_size^2 + 1 rows.  Runs on the
+        host, once per load.  Copying table 0 to every layer is left to the model (one_peace_classify)."""
+        prefix = f"{name}." if name else ""
+        key = prefix + "rel_pos_table_list.0.weight"
+        if prefix + "rel_pos_table.weight" in state_dict:
+            state_dict[key] = state_dict.pop(prefix + "rel_pos_table.weight")
+        if self.rel_pos_table_list is not None and key in state_dict and \
+                (2 * self.rel_bucket_size - 1) ** 2 + 3 > state_dict[key].shape[0]:
+            table = state_dict[key]
+            src = int((table.shape[0] - 3) ** 0.5)
+            new = geometric_sequence_interpolation(src, 2 * self.rel_bucket_size - 1, table[:-3].cpu(), table.shape[1])
+            state_dict[key] = torch.cat([new.to(table), table[-3:]], dim=0)
+            state_dict[prefix + "rp_bucket"] = self.rp_bucket.clone()
+        pk = prefix + "pos_embed"
+        if pk in state_dict and self.bucket_size ** 2 + 1 > state_dict[pk].shape[0]:
+            pe = state_dict[pk]
+            n = int((pe.shape[0] - 1) ** 0.5)
+            old = pe[1:].reshape(1, n, n, -1).permute(0, 3, 1, 2)
+            new = F.interpolate(old, size=(self.bucket_size, self.bucket_size), mode="bicubic")
+            state_dict[pk] = torch.cat([pe[:1], new.permute(0, 2, 3, 1).reshape(self.bucket_size ** 2, -1)], dim=0)
+            state_dict[prefix + "position_idx"] = self.position_idx.clone()
 
     def _resize_matrix(self, w, device):
         key = (w, str(device))

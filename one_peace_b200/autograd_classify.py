@@ -1,5 +1,6 @@
 """Training path of the classification head (models/one_peace/one_peace_base.py:132-235, OnePeaceClassifyHead with attention
-pooling) and of the classification criteria (criterions/classify_loss.py, criterions/hinge_loss.py), as
+pooling) and of the classification and grounding criteria (criterions/classify_loss.py, criterions/hinge_loss.py,
+criterions/refcoco_loss.py), as
 ``torch.autograd.Function`` nodes whose forward and backward are sm_90a kernels:
 
     per-token features [B, S, d] (after the modality's final LayerNorm; CLS row dropped)
@@ -171,3 +172,25 @@ class ClassifyLossFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, g_loss, _g1, _g2):
         return (ctx.dl * g_loss.to(torch.float32)).to(ctx.dtype), None, None, None, None, None
+
+
+class RefcocoLossFn(torch.autograd.Function):
+    """logits [B, 4] (any row pitch), targets [B, 4], nsentences -> (loss, L1 part, n_valid) of refcoco_criterion
+    (criterions/refcoco_loss.py:36-46); the gradient is computed in the same launch (opb_refcoco_loss) and scaled by the
+    upstream gradient in the backward.  The loss is NaN when no row is valid while the gradient stays the finite L1 part."""
+
+    @staticmethod
+    def forward(ctx, logits, targets, nsentences):
+        x = logits.detach()
+        if x.dtype != torch.float32 or x.stride(1) != 1:
+            x = x.float().contiguous()
+        out, _, _, dl = K.refcoco_loss(x, targets.detach(), nsentences)
+        ctx.dl = dl[:, :logits.shape[1]]
+        ctx.dtype = logits.dtype
+        l1, n_valid = out[1], out[2]
+        ctx.mark_non_differentiable(l1, n_valid)
+        return out[0], l1, n_valid
+
+    @staticmethod
+    def backward(ctx, g_loss, _g1, _g2):
+        return (ctx.dl * g_loss.to(torch.float32)).to(ctx.dtype), None, None

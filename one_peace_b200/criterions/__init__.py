@@ -4,3 +4,4 @@ from .image_text_pretrain_loss import ImageTextPretrainLossCriterion  # noqa: F4
 from .audio_text_pretrain_loss import AudioTextPretrainLossCriterion  # noqa: F401
 from .classify_loss import ClassifyCriterion  # noqa: F401
 from .hinge_loss import HingeLoss  # noqa: F401
+from .refcoco_loss import RefCOCOCriterion  # noqa: F401

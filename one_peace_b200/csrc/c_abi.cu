@@ -434,4 +434,15 @@ int opb_classify_loss(const float* logits, int64_t ld, int rows, int n_valid, in
                             row_correct, out2, ticket, static_cast<cudaStream_t>(stream));
 }
 
+int opb_refcoco_loss(const float* logits, int64_t ld, const float* targets, int B, int nsentences, float* out, int* valid,
+                     float* giou, float* dlogits, void* stream) {
+  if (!logits || !targets || !out || !valid || !giou || !dlogits) return OPB_ERR_INVALID;
+  return opb::refcoco_loss(logits, ld, targets, B, nsentences, out, valid, giou, dlogits, static_cast<cudaStream_t>(stream));
+}
+
+int opb_iou_acc(const float* hyps, int64_t ld_h, const float* refs, int64_t ld_r, int n, int* hits, int* row_hit, void* stream) {
+  if (!hyps || !refs || !hits) return OPB_ERR_INVALID;
+  return opb::iou_acc(hyps, ld_h, refs, ld_r, n, hits, row_hit, static_cast<cudaStream_t>(stream));
+}
+
 }  // extern "C"

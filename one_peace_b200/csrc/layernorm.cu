@@ -211,9 +211,9 @@ static int launch_ln(const LnArgs& a, cudaStream_t stream) {
   else if (need <= 4) OPB_LN(4);
   else if (need <= 6) OPB_LN(6);
   else if (need <= 8) OPB_LN(8);
-  else if (sizeof(TIn) == 2 && need <= 12) OPB_LN(12);
+  else if (need <= 12) OPB_LN(12);             // fp32 rows up to 3072: the classifier of a head_scale_ratio 2 head at d 1536
   else if (sizeof(TIn) == 2 && need <= 24) OPB_LN(24);
-  else return OPB_ERR_UNSUPPORTED;            // rows wider than 6144 (bf16) / 2048 (fp32) are not on this path
+  else return OPB_ERR_UNSUPPORTED;            // rows wider than 6144 (bf16) / 3072 (fp32) are not on this path
 #undef OPB_LN
   return cudaGetLastError() == cudaSuccess ? OPB_OK : OPB_ERR_CUDA;
 }

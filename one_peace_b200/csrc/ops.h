@@ -158,4 +158,9 @@ int classify_loss(const float* logits, long ld, int rows, int n_valid, int mode,
                   long ld_t, float eps, int num_choices, float* row_loss, float* dlogits, float* row_correct, float* out2,
                   unsigned int* ticket, cudaStream_t stream);
 
+// csrc/grounding.cu: the box loss of refcoco_criterion and the hit counter of IouAcc
+int refcoco_loss(const float* logits, long ld, const float* targets, int B, int nsentences, float* out, int* valid, float* giou,
+                 float* dlogits, cudaStream_t stream);
+int iou_acc(const float* hyps, long ld_h, const float* refs, long ld_r, int n, int* hits, int* row_hit, cudaStream_t stream);
+
 }  // namespace opb

@@ -856,3 +856,43 @@ def classify_loss(logits, n_valid, mode, labels=None, targets=None, eps=0.0, num
     _lib.check(st, "opb_classify_loss")
     _count()
     return row_loss, dlogits, row_correct, out2
+
+
+# ----------------------------------------------------------------------------------------------------------------
+# visual grounding (csrc/grounding.cu)
+# ----------------------------------------------------------------------------------------------------------------
+def refcoco_loss(logits, targets, nsentences):
+    """logits fp32 [B, >= 4] (unit column stride, free row pitch ld; columns past 4 are never read), targets [B, 4] ->
+    (out fp32 [3] = {loss, L1 part, n_valid}, valid int32 [B], giou fp32 [B], dlogits fp32 [B, ld] = d loss / d logits with
+    zero pad columns).  The loss is NaN when no row is valid; dlogits stays finite (the L1 part)."""
+    _need_cuda(logits, targets)
+    assert logits.dtype == torch.float32 and logits.dim() == 2 and logits.stride(1) == 1
+    B, ld = logits.shape[0], logits.stride(0)
+    dev = logits.device
+    t = targets.to(torch.float32).contiguous()
+    assert t.shape == (B, 4)
+    out = torch.empty(3, dtype=torch.float32, device=dev)
+    valid = torch.empty(B, dtype=torch.int32, device=dev)
+    giou = torch.empty(B, dtype=torch.float32, device=dev)
+    dlogits = torch.empty(B, ld, dtype=torch.float32, device=dev)
+    st = _lib.load().opb_refcoco_loss(logits.data_ptr(), ld, t.data_ptr(), B, int(nsentences), out.data_ptr(), valid.data_ptr(),
+                                      giou.data_ptr(), dlogits.data_ptr(), _stream())
+    _lib.check(st, "opb_refcoco_loss")
+    _count()
+    return out, valid, giou, dlogits
+
+
+def iou_acc(hyps, refs, hits, row_hit=None):
+    """hits int32 [1] += IoU >= 0.5 hits of hyps / refs fp32 [n, 4] (metrics/iou_acc.py:20-32); asynchronous.  row_hit: optional
+    int32 [n] receiving the per-row flag."""
+    _need_cuda(hyps, refs, hits, row_hit)
+    assert hyps.dtype == torch.float32 and refs.dtype == torch.float32 and hyps.stride(1) == 1 and refs.stride(1) == 1
+    assert hyps.shape == refs.shape and hyps.shape[1] == 4
+    assert hits.dtype == torch.int32 and hits.numel() >= 1
+    if row_hit is not None:
+        assert row_hit.dtype == torch.int32 and row_hit.is_contiguous() and row_hit.numel() == hyps.shape[0]
+    st = _lib.load().opb_iou_acc(hyps.data_ptr(), hyps.stride(0), refs.data_ptr(), refs.stride(0), hyps.shape[0], hits.data_ptr(),
+                                 _ptr(row_hit), _stream())
+    _lib.check(st, "opb_iou_acc")
+    _count()
+    return hits

@@ -1,1 +1,2 @@
 from .recall import Recall  # noqa: F401
+from .iou_acc import IouAcc  # noqa: F401

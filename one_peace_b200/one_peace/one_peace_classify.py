@@ -143,6 +143,8 @@ class OnePeaceClassifyModel(OnePeaceBaseModel):
         prefix = f"{name}." if name else ""
         for m in self.modalities:
             p = f"{prefix}encoder_wrapper.{m}_adapter."
+            if m == "image":                       # a 256^2 checkpoint's tables resized for the configured image size
+                self.encoder_wrapper.image_adapter.upgrade_state_dict_named(state_dict, p[:-1])
             if p + "rel_pos_table.weight" in state_dict:
                 state_dict[p + "rel_pos_table_list.0.weight"] = state_dict.pop(p + "rel_pos_table.weight")
             if p + "rel_pos_table_list.0.weight" in state_dict and p + "rel_pos_table_list.1.weight" not in state_dict:
