@@ -514,6 +514,44 @@ int opb_refcoco_loss(const float* logits, int64_t ld, const float* targets, int 
                      float* giou, float* dlogits, void* stream);
 int opb_iou_acc(const float* hyps, int64_t ld_h, const float* refs, int64_t ld_r, int n, int* hits, int* row_hit, void* stream);
 
+/* ------------------------------------------------------------------------------------------------------------------
+ * Classification evaluation (Accuracy and MAP).
+ *   opb_argmax_hits   : metrics/accuracy.py:20-25: hyp[r] = torch.argmax(logits[r, 0:C]) as int64 (the first maximal
+ *                       index; a NaN is the maximum, so the first NaN wins; bf16 compares after its exact up-cast) and
+ *                       score[r] fp32 = the row's hit: tmode 0 int64 labels [n] -> 1 / 0 for hyp == label; tmode 1 fp32
+ *                       labels [n] -> 1 / 0 for float(hyp) == label (torch.eq's promotion); tmode 2 soft scores fp32
+ *                       [n, ldt] -> targets[r, hyp] exactly.  logits fp32 (dtype OPB_F32) or bf16 (OPB_BF16) at element
+ *                       (r, j) = logits[r * ld + j * cs], so padded rows and column-strided views are read in place.
+ *                       One warp per row for C > 8, one thread per row for C <= 8.  Status 1 for n <= 0, C outside
+ *                       [1, 4096], ld or cs < 1, an unknown dtype / tmode, ldt < C with tmode 2, or a null pointer.
+ *   opb_sum_f64       : out[0] = sum of x fp32 [n] in fp64 in a fixed order (one CTA): bit-identical on every run.
+ *                       Status 1 for n <= 0 or a null pointer.
+ *   opb_sigmoid_pack  : metrics/map.py:20-23 and the torch.sigmoid of :34: for r < n, j < C, with o = (row_offset + r) * C + j,
+ *                       probs[o] = 1 / (1 + expf(-x)) in IEEE fp32 (torch.sigmoid's CUDA fp32 result bit for bit; bf16 is
+ *                       up-cast first) and labels[o] = uint8(targets[r * ldt + j] == 1).  flags int32 [2] (the caller
+ *                       zeroes it once): flags[0] += number of targets outside {0, 1}, flags[1] += number of NaN
+ *                       probabilities.  Status 1 for n <= 0, C outside [1, 4096], ld or cs < 1, ldt < C, row_offset < 0,
+ *                       an unknown dtype or a null pointer.
+ *   opb_average_precision : sklearn.metrics.average_precision_score(labels, probs, average=None) and the np.mean of
+ *                       metrics/map.py:43.  probs fp32 [N, C] in [0, 1] (values outside are clamped into it), labels uint8
+ *                       [N, C] (non-zero = positive), 1 <= N < 2^24, 1 <= C <= 4096, N * C < 2^31.  Per class: sort by
+ *                       probability, descending; group equal probabilities; ap[c] = sum over groups g of
+ *                       pos_g * TP_g / (TP_g + FP_g) / P_c with TP / FP counted through g, 0 when P_c = 0.  Counts are exact
+ *                       integers, each group's term is formed in fp64 and the terms are summed in a fixed order; mean[0] is
+ *                       the fp64 mean of ap in class order; npos int64 [C] = P_c.  Device-wide LSD radix sort of
+ *                       class-major 64-bit keys in the workspace of opb_average_precision_ws_bytes(N, C) bytes (-1 for a
+ *                       shape outside the range above).  Status 1 for a shape outside that range, a smaller workspace or a
+ *                       null pointer.
+ * ------------------------------------------------------------------------------------------------------------------ */
+int opb_argmax_hits(const void* logits, int dtype, int64_t ld, int64_t cs, int n, int C, const void* targets, int tmode,
+                    int64_t ldt, int64_t* hyp, float* score, void* stream);
+int opb_sum_f64(const float* x, int64_t n, double* out, void* stream);
+int opb_sigmoid_pack(const void* logits, int dtype, int64_t ld, int64_t cs, const float* targets, int64_t ldt, int n, int C,
+                     float* probs, uint8_t* labels, int64_t row_offset, int* flags, void* stream);
+int64_t opb_average_precision_ws_bytes(int N, int C);
+int opb_average_precision(const float* probs, const uint8_t* labels, int N, int C, void* ws, int64_t ws_bytes, double* ap,
+                          double* mean, int64_t* npos, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -105,6 +105,14 @@ SIGNATURES.update({
                                   c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "opb_refcoco_loss": (c_int, [c_void_p, c_int64, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "opb_iou_acc": (c_int, [c_void_p, c_int64, c_void_p, c_int64, c_int, c_void_p, c_void_p, c_void_p]),
+    "opb_argmax_hits": (c_int, [c_void_p, c_int, c_int64, c_int64, c_int, c_int, c_void_p, c_int, c_int64, c_void_p, c_void_p,
+                                c_void_p]),
+    "opb_sum_f64": (c_int, [c_void_p, c_int64, c_void_p, c_void_p]),
+    "opb_sigmoid_pack": (c_int, [c_void_p, c_int, c_int64, c_int64, c_void_p, c_int64, c_int, c_int, c_void_p, c_void_p, c_int64,
+                                 c_void_p, c_void_p]),
+    "opb_average_precision_ws_bytes": (c_int64, [c_int, c_int]),
+    "opb_average_precision": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_int64, c_void_p, c_void_p, c_void_p,
+                                      c_void_p]),
 })
 
 

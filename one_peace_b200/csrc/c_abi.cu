@@ -445,4 +445,30 @@ int opb_iou_acc(const float* hyps, int64_t ld_h, const float* refs, int64_t ld_r
   return opb::iou_acc(hyps, ld_h, refs, ld_r, n, hits, row_hit, static_cast<cudaStream_t>(stream));
 }
 
+int opb_argmax_hits(const void* logits, int dtype, int64_t ld, int64_t cs, int n, int C, const void* targets, int tmode,
+                    int64_t ldt, int64_t* hyp, float* score, void* stream) {
+  if (!logits || !targets || !hyp || !score) return OPB_ERR_INVALID;
+  return opb::argmax_hits(logits, dtype, ld, cs, n, C, targets, tmode, ldt, hyp, score, static_cast<cudaStream_t>(stream));
+}
+
+int opb_sum_f64(const float* x, int64_t n, double* out, void* stream) {
+  if (!x || !out) return OPB_ERR_INVALID;
+  return opb::sum_f64(x, n, out, static_cast<cudaStream_t>(stream));
+}
+
+int opb_sigmoid_pack(const void* logits, int dtype, int64_t ld, int64_t cs, const float* targets, int64_t ldt, int n, int C,
+                     float* probs, uint8_t* labels, int64_t row_offset, int* flags, void* stream) {
+  if (!logits || !targets || !probs || !labels || !flags) return OPB_ERR_INVALID;
+  return opb::sigmoid_pack(logits, dtype, ld, cs, targets, ldt, n, C, probs, labels, row_offset, flags,
+                           static_cast<cudaStream_t>(stream));
+}
+
+int64_t opb_average_precision_ws_bytes(int N, int C) { return opb::average_precision_ws_bytes(N, C); }
+
+int opb_average_precision(const float* probs, const uint8_t* labels, int N, int C, void* ws, int64_t ws_bytes, double* ap,
+                          double* mean, int64_t* npos, void* stream) {
+  if (!probs || !labels || !ws || !ap || !mean || !npos) return OPB_ERR_INVALID;
+  return opb::average_precision(probs, labels, N, C, ws, ws_bytes, ap, mean, npos, static_cast<cudaStream_t>(stream));
+}
+
 }  // extern "C"

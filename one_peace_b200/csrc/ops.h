@@ -163,4 +163,14 @@ int refcoco_loss(const float* logits, long ld, const float* targets, int B, int 
                  float* dlogits, cudaStream_t stream);
 int iou_acc(const float* hyps, long ld_h, const float* refs, long ld_r, int n, int* hits, int* row_hit, cudaStream_t stream);
 
+// csrc/metrics.cu: the argmax hit counter of Accuracy, the sigmoid packing of MAP and the per-class average precision
+int argmax_hits(const void* logits, int dtype, long ld, long cs, int n, int C, const void* targets, int tmode, long ldt,
+                int64_t* hyp, float* score, cudaStream_t stream);
+int sum_f64(const float* x, long n, double* out, cudaStream_t stream);
+int sigmoid_pack(const void* logits, int dtype, long ld, long cs, const float* targets, long ldt, int n, int C, float* probs,
+                 uint8_t* labels, long row_offset, int* flags, cudaStream_t stream);
+long average_precision_ws_bytes(int N, int C);
+int average_precision(const float* probs, const uint8_t* labels, int N, int C, void* ws, long ws_bytes, double* ap,
+                      double* mean, int64_t* npos, cudaStream_t stream);
+
 }  // namespace opb

@@ -896,3 +896,96 @@ def iou_acc(hyps, refs, hits, row_hit=None):
     _lib.check(st, "opb_iou_acc")
     _count()
     return hits
+
+
+# ----------------------------------------------------------------------------------------------------------------
+# classification evaluation (csrc/metrics.cu)
+# ----------------------------------------------------------------------------------------------------------------
+def _view2d(x):
+    """(dtype tag, row stride, column stride) of a 2-D fp32 / bf16 view, read in place (no copy of padded or strided rows)."""
+    assert x.dim() == 2
+    return _dt(x), max(x.stride(0), 1), max(x.stride(1), 1)
+
+
+def argmax_hits(logits, targets, hyp=None, score=None):
+    """metrics/accuracy.py:20-25: hyp int64 [n] = torch.argmax(logits, 1) and score fp32 [n] = the row's hit.  logits fp32 / bf16
+    [n, C] with any strides; targets int64 labels [n], fp32 labels [n] (compared as torch.eq does) or fp32 soft scores [n, >= C]
+    (score = targets[r, hyp]).  Asynchronous."""
+    _need_cuda(logits, targets, hyp, score)
+    dt, ld, cs = _view2d(logits)
+    n, C = logits.shape
+    if targets.dim() == 2:
+        t = targets if targets.dtype == torch.float32 and targets.stride(1) == 1 else targets.to(torch.float32).contiguous()
+        assert t.shape[0] == n and t.shape[1] >= C
+        tmode, ldt = 2, max(t.stride(0), 1)
+    else:
+        assert targets.dim() == 1 and targets.shape[0] == n
+        if targets.dtype == torch.int64:
+            t, tmode = targets.contiguous(), 0
+        elif targets.is_floating_point() or targets.dtype == torch.bool:
+            t, tmode = targets.to(torch.float32).contiguous(), 1
+        else:
+            t, tmode = targets.to(torch.int64).contiguous(), 0
+        ldt = 0
+    dev = logits.device
+    hyp = torch.empty(n, dtype=torch.int64, device=dev) if hyp is None else hyp
+    score = torch.empty(n, dtype=torch.float32, device=dev) if score is None else score
+    assert hyp.dtype == torch.int64 and hyp.is_contiguous() and hyp.numel() >= n
+    assert score.dtype == torch.float32 and score.is_contiguous() and score.numel() >= n
+    st = _lib.load().opb_argmax_hits(logits.data_ptr(), dt, ld, cs, n, C, t.data_ptr(), tmode, ldt, hyp.data_ptr(),
+                                     score.data_ptr(), _stream())
+    _lib.check(st, "opb_argmax_hits")
+    _count()
+    return hyp, score
+
+
+def sum_f64(x, out=None):
+    """fp64 [1] = sum of x fp32 [n] in a fixed order (bit-identical on every run)."""
+    _need_cuda(x, out)
+    assert x.dtype == torch.float32 and x.is_contiguous()
+    out = torch.empty(1, dtype=torch.float64, device=x.device) if out is None else out
+    st = _lib.load().opb_sum_f64(x.data_ptr(), x.numel(), out.data_ptr(), _stream())
+    _lib.check(st, "opb_sum_f64")
+    _count()
+    return out
+
+
+def sigmoid_pack(logits, targets, probs, labels, row_offset, flags):
+    """metrics/map.py:20-23 + the sigmoid of :34: probs[row_offset + r] = torch.sigmoid(float(logits[r])) bit for bit, labels
+    uint8 = (targets == 1), flags int32 [2] += (targets outside {0, 1}, NaN probabilities).  logits fp32 / bf16 [n, C], any
+    strides; targets fp32 [n, C]; probs fp32 / labels uint8 [>= row_offset + n, C] contiguous.  Asynchronous."""
+    _need_cuda(logits, targets, probs, labels, flags)
+    dt, ld, cs = _view2d(logits)
+    n, C = logits.shape
+    t = targets if targets.dtype == torch.float32 and targets.stride(1) == 1 else targets.to(torch.float32).contiguous()
+    assert t.shape == (n, C)
+    assert probs.dtype == torch.float32 and probs.is_contiguous() and probs.shape[1] == C and probs.shape[0] >= row_offset + n
+    assert labels.dtype == torch.uint8 and labels.is_contiguous() and labels.shape == probs.shape
+    assert flags.dtype == torch.int32 and flags.numel() >= 2
+    st = _lib.load().opb_sigmoid_pack(logits.data_ptr(), dt, ld, cs, t.data_ptr(), max(t.stride(0), 1), n, C, probs.data_ptr(),
+                                      labels.data_ptr(), row_offset, flags.data_ptr(), _stream())
+    _lib.check(st, "opb_sigmoid_pack")
+    _count()
+
+
+def average_precision(probs, labels):
+    """sklearn.metrics.average_precision_score(labels, probs, average=None) and its mean: probs fp32 [N, C] in [0, 1], labels
+    uint8 [N, C] -> (ap fp64 [C], mean fp64 [1], npos int64 [C]); ap is 0 for a class without positives."""
+    _need_cuda(probs, labels)
+    assert probs.dtype == torch.float32 and probs.is_contiguous() and labels.dtype == torch.uint8 and labels.is_contiguous()
+    assert probs.dim() == 2 and labels.shape == probs.shape
+    N, C = probs.shape
+    lib = _lib.load()
+    nbytes = lib.opb_average_precision_ws_bytes(N, C)
+    if nbytes < 0:
+        raise RuntimeError(f"opb_average_precision: shape {N} x {C} is outside 1 <= N < 2^24, 1 <= C <= 4096, N * C < 2^31")
+    dev = probs.device
+    ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+    ap = torch.empty(C, dtype=torch.float64, device=dev)
+    mean = torch.empty(1, dtype=torch.float64, device=dev)
+    npos = torch.empty(C, dtype=torch.int64, device=dev)
+    st = lib.opb_average_precision(probs.data_ptr(), labels.data_ptr(), N, C, ws.data_ptr(), nbytes, ap.data_ptr(),
+                                   mean.data_ptr(), npos.data_ptr(), _stream())
+    _lib.check(st, "opb_average_precision")
+    _count(4 + 3 * ((31 + max(C - 1, 0).bit_length() + 7) // 8))
+    return ap, mean, npos
