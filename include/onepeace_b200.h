@@ -303,6 +303,28 @@ int opb_adam_multi_step(const void* tensors, const int32_t* chunk_tensor, const 
 int opb_grad_norm_clip(const void* tensors, const int32_t* chunk_tensor, const int64_t* chunk_off, int n_chunks,
                        float* partial, float multiply_factor, float max_norm, float* out2, void* stream);
 
+/*
+ * Fused multi-tensor Adan step (optim/adan.py:146-223, registered as `adan` at :53; one launch per step, same
+ * 8192-element chunk table as opb_adam_multi_step).  Per element, fp32, each operation rounded on its own:
+ *   g = grad * grad_scale;  diff = g - pre_grad (0 on a parameter's first step, :197-198);  u = g + b2 diff (:205)
+ *   m = b1 m + (1-b1) g;  n = b2 n + (1-b2) diff;  v = b3 v + (1-b3) u^2                              (:206-208)
+ *   upd = (m / bc1 + (b2 n) / bc2) / (sqrt(v) / sqrt_bc3 + eps)                                       (:210-211)
+ *   no_prox = 0: p = (p - lr upd) / (1 + lr wd);  no_prox = 1: p = p (1 - lr wd) - lr upd            (:213-218)
+ *   pre_grad = g                                                                                       (:220)
+ *   tensors       device array of records {void* p; const void* g; float* m (exp_avg); float* n (exp_avg_diff);
+ *                 float* v (exp_avg_sq); float* pre_grad; float* master; int64 numel; int32 group, p_dtype, g_dtype,
+ *                 first}  (80 bytes each; dtype 0 fp32, 1 bf16; master NULL = up-cast p; first = 1: diff = 0 and
+ *                 pre_grad is only written, it may hold anything)
+ *   lr, wd, no_prox, bc1 (1 - b1^t), bc2 (1 - b2^t), sqrt_bc3 (sqrt(1 - b3^t))   HOST arrays [n_groups <= 128], t the
+ *                 group's step count (:160-169)
+ *   grad_scale    device scalar multiplied into every gradient (NULL = 1); pre_grad stores the scaled gradient
+ * Null pointers give OPB_ERR_INVALID and a group count outside 1..128 OPB_ERR_UNSUPPORTED, before any CUDA call.
+ */
+int opb_adan_multi_step(const void* tensors, const int32_t* chunk_tensor, const int64_t* chunk_off, int n_chunks,
+                        const float* lr, const float* wd, const int32_t* no_prox, const float* bc1, const float* bc2,
+                        const float* sqrt_bc3, int n_groups, float beta1, float beta2, float beta3, float eps,
+                        const float* grad_scale, void* stream);
+
 /* ------------------------------------------------------------------------------------------------------------------
  * Backward pass of the encoder layer (autograd of models/transformer/transformer_layer.py:165-228 and
  * multihead_attention.py:103-126; the reference relies on torch autograd, these are the hand-written adjoints).

@@ -59,6 +59,8 @@ SIGNATURES = {
     "opb_adam_multi_step": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int, c_float,
                                     c_float, c_float, c_void_p, c_void_p]),
     "opb_grad_norm_clip": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_float, c_float, c_void_p, c_void_p]),
+    "opb_adan_multi_step": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                    c_void_p, c_int, c_float, c_float, c_float, c_float, c_void_p, c_void_p]),
 }
 
 SIGNATURES.update({

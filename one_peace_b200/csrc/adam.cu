@@ -145,6 +145,112 @@ int adam_multi_step(const void* tensors, const int* chunk_tensor, const long* ch
   return cudaGetLastError() == cudaSuccess ? OPB_OK : OPB_ERR_CUDA;
 }
 
+// ---- Adan (optim/adan.py:146-223), same chunk table and launch shape as Adam ----
+//   per element, fp32:   g = grad * grad_scale ;  diff = g - (first ? g : pre) ;  u = g + b2 diff
+//                        m = b1 m + (1-b1) g ;  n = b2 n + (1-b2) diff ;  v = b3 v + (1-b3) u^2
+//                        upd = (m / bc1 + (b2 n) / bc2) / (sqrt(v) / sqrt(bc3) + eps)
+//                        proximal (no_prox = 0):  p = (p - lr upd) / (1 + lr wd)      (:216-218)
+//                        no_prox = 1:             p = p (1 - lr wd) - lr upd          (:213-215)
+//                        pre = g                                                       (:220, the scaled gradient)
+// Each operation is rounded on its own, in the reference's order.  Traffic: read g + p + m/n/v/pre (16), write
+// m/n/v/pre (16) + p: 38 B / parameter with bf16 p and g, 44 B with fp32 p and g or with a master copy.
+struct AdanCoef {
+  float b1, b2, b3, c1, c2, c3, eps, lr, decay, bc1, bc2, sbc3;
+  bool no_prox;
+};
+
+OPB_DEVICE void adan_math(float& p, float g, float& pre, float& m, float& n, float& v, bool first, const AdanCoef& c) {
+  // first step: pre_grad = g (:197-198), so diff = g - g: 0, or NaN for a non-finite g, as in the reference
+  const float diff = __fsub_rn(g, first ? g : pre);
+  const float u = __fadd_rn(g, __fmul_rn(c.b2, diff));
+  m = __fadd_rn(__fmul_rn(m, c.b1), __fmul_rn(g, c.c1));
+  n = __fadd_rn(__fmul_rn(n, c.b2), __fmul_rn(diff, c.c2));
+  v = __fadd_rn(__fmul_rn(v, c.b3), __fmul_rn(__fmul_rn(c.c3, u), u));   // addcmul_: value * t1 * t2
+  const float denom = __fadd_rn(__fdiv_rn(sqrtf(v), c.sbc3), c.eps);
+  const float upd = __fdiv_rn(__fadd_rn(__fdiv_rn(m, c.bc1), __fdiv_rn(__fmul_rn(c.b2, n), c.bc2)), denom);
+  if (c.no_prox) p = __fadd_rn(__fmul_rn(p, c.decay), __fmul_rn(-c.lr, upd));
+  else p = __fdiv_rn(__fadd_rn(p, __fmul_rn(-c.lr, upd)), c.decay);
+  pre = g;
+}
+
+template <typename TP, typename TG>
+__device__ void adan_chunk(const AdanTensor& t, long off, long cnt, float gscale, const AdanCoef& c) {
+  TP* p = reinterpret_cast<TP*>(t.p) + off;
+  const TG* g = reinterpret_cast<const TG*>(t.g) + off;
+  float* m = t.m + off;
+  float* n = t.n + off;
+  float* v = t.v + off;
+  float* pre = t.pre + off;
+  float* master = t.master ? t.master + off : nullptr;
+  const bool first = t.first != 0;
+  const bool vec_ok = ((reinterpret_cast<uintptr_t>(p) | reinterpret_cast<uintptr_t>(g) | reinterpret_cast<uintptr_t>(m) |
+                        reinterpret_cast<uintptr_t>(n) | reinterpret_cast<uintptr_t>(v) | reinterpret_cast<uintptr_t>(pre) |
+                        reinterpret_cast<uintptr_t>(master)) & 15) == 0;
+  long i0 = threadIdx.x;
+  if (vec_ok) {
+    const long n4 = cnt & ~3L;
+    for (long i = threadIdx.x * 4L; i < n4; i += kAdamThreads * 4L) {
+      float pv[4], gv[4], mv[4], nv[4], vv[4], qv[4] = {0.f, 0.f, 0.f, 0.f};
+      if (master) ld4<float>(master + i, pv); else ld4<TP>(p + i, pv);
+      ld4<TG>(g + i, gv);
+      ld4<float>(m + i, mv);
+      ld4<float>(n + i, nv);
+      ld4<float>(v + i, vv);
+      if (!first) ld4<float>(pre + i, qv);
+#pragma unroll
+      for (int e = 0; e < 4; ++e) adan_math(pv[e], __fmul_rn(gv[e], gscale), qv[e], mv[e], nv[e], vv[e], first, c);
+      st4<float>(m + i, mv);
+      st4<float>(n + i, nv);
+      st4<float>(v + i, vv);
+      st4<float>(pre + i, qv);
+      if (master) st4<float>(master + i, pv);
+      st4<TP>(p + i, pv);
+    }
+    i0 = n4 + threadIdx.x;
+  }
+  for (long i = i0; i < cnt; i += kAdamThreads) {
+    float pv = master ? master[i] : ld1<TP>(p, i);
+    float qv = first ? 0.f : pre[i];
+    float mv = m[i], nv = n[i], vv = v[i];
+    adan_math(pv, __fmul_rn(ld1<TG>(g, i), gscale), qv, mv, nv, vv, first, c);
+    m[i] = mv; n[i] = nv; v[i] = vv; pre[i] = qv;
+    if (master) master[i] = pv;
+    st1<TP>(p, i, pv);
+  }
+}
+
+__global__ void __launch_bounds__(kAdamThreads)
+adan_multi_kernel(const AdanTensor* __restrict__ tensors, const int* __restrict__ chunk_tensor,
+                  const long* __restrict__ chunk_off, const AdanGroups groups, const float* __restrict__ grad_scale) {
+  const int ci = blockIdx.x;
+  const AdanTensor t = tensors[chunk_tensor[ci]];
+  const long off = chunk_off[ci];
+  long cnt = t.numel - off;
+  if (cnt > kChunk) cnt = kChunk;
+  const float gscale = grad_scale ? *grad_scale : 1.f;
+  const int gi = t.group;
+  AdanCoef c;
+  c.b1 = groups.beta1; c.b2 = groups.beta2; c.b3 = groups.beta3; c.eps = groups.eps;
+  c.c1 = 1.f - c.b1; c.c2 = 1.f - c.b2; c.c3 = 1.f - c.b3;
+  c.lr = groups.lr[gi];
+  c.no_prox = groups.no_prox[gi] != 0;
+  const float lr_wd = __fmul_rn(c.lr, groups.wd[gi]);
+  c.decay = c.no_prox ? __fsub_rn(1.f, lr_wd) : __fadd_rn(1.f, lr_wd);
+  c.bc1 = groups.bc1[gi]; c.bc2 = groups.bc2[gi]; c.sbc3 = groups.sqrt_bc3[gi];
+  if (t.p_dtype == 0 && t.g_dtype == 0) adan_chunk<float, float>(t, off, cnt, gscale, c);
+  else if (t.p_dtype == 1 && t.g_dtype == 1) adan_chunk<__nv_bfloat16, __nv_bfloat16>(t, off, cnt, gscale, c);
+  else if (t.p_dtype == 1 && t.g_dtype == 0) adan_chunk<__nv_bfloat16, float>(t, off, cnt, gscale, c);
+  else adan_chunk<float, __nv_bfloat16>(t, off, cnt, gscale, c);
+}
+
+int adan_multi_step(const void* tensors, const int* chunk_tensor, const long* chunk_off, int n_chunks,
+                    const AdanGroups& groups, const float* grad_scale, cudaStream_t stream) {
+  if (n_chunks <= 0) return OPB_ERR_INVALID;
+  adan_multi_kernel<<<n_chunks, kAdamThreads, 0, stream>>>(reinterpret_cast<const AdanTensor*>(tensors), chunk_tensor,
+                                                           chunk_off, groups, grad_scale);
+  return cudaGetLastError() == cudaSuccess ? OPB_OK : OPB_ERR_CUDA;
+}
+
 // ---- grad norm: stage 1 = per-CTA sum of squares, stage 2 = ordered fp64 sum + clip coefficient ----
 // CTA b owns chunks b, b + grid, b + 2 grid, ... (fixed assignment); every thread adds ITS elements of those chunks in that
 // order into one register and the CTA reduces once at the end (fixed tree), so identical gradients give bit-identical norms

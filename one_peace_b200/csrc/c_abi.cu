@@ -244,6 +244,22 @@ int opb_adam_multi_step(const void* tensors, const int32_t* chunk_tensor, const 
                               static_cast<cudaStream_t>(stream));
 }
 
+int opb_adan_multi_step(const void* tensors, const int32_t* chunk_tensor, const int64_t* chunk_off, int n_chunks,
+                        const float* lr, const float* wd, const int32_t* no_prox, const float* bc1, const float* bc2,
+                        const float* sqrt_bc3, int n_groups, float beta1, float beta2, float beta3, float eps,
+                        const float* grad_scale, void* stream) {
+  if (!tensors || !chunk_tensor || !chunk_off || !lr || !wd || !no_prox || !bc1 || !bc2 || !sqrt_bc3) return OPB_ERR_INVALID;
+  if (n_groups <= 0 || n_groups > opb::kAdanMaxGroups) return OPB_ERR_UNSUPPORTED;
+  opb::AdanGroups g;
+  for (int i = 0; i < n_groups; ++i) {
+    g.lr[i] = lr[i]; g.wd[i] = wd[i]; g.no_prox[i] = no_prox[i];
+    g.bc1[i] = bc1[i]; g.bc2[i] = bc2[i]; g.sqrt_bc3[i] = sqrt_bc3[i];
+  }
+  g.beta1 = beta1; g.beta2 = beta2; g.beta3 = beta3; g.eps = eps;
+  return opb::adan_multi_step(tensors, chunk_tensor, reinterpret_cast<const long*>(chunk_off), n_chunks, g, grad_scale,
+                              static_cast<cudaStream_t>(stream));
+}
+
 int opb_grad_norm_clip(const void* tensors, const int32_t* chunk_tensor, const int64_t* chunk_off, int n_chunks,
                        float* partial, float multiply_factor, float max_norm, float* out2, void* stream) {
   if (!tensors || !chunk_tensor || !chunk_off || !partial || !out2) return OPB_ERR_INVALID;

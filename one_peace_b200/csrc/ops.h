@@ -96,6 +96,34 @@ int adam_multi_step(const void* tensors, const int* chunk_tensor, const long* ch
 int grad_norm_clip(const void* tensors, const int* chunk_tensor, const long* chunk_off, int n_chunks, float* partial,
                    float multiply_factor, float max_norm, float* out2, cudaStream_t stream);
 
+// Adan (optim/adan.py:146-223): one entry per parameter tensor (device-resident table, 80 bytes; mirrored in optim/adan.py)
+struct AdanTensor {
+  void* p;         // parameter (fp32 or bf16)
+  const void* g;   // gradient (fp32 or bf16)
+  float* m;        // exp_avg
+  float* n;        // exp_avg_diff
+  float* v;        // exp_avg_sq
+  float* pre;      // pre_grad (the previous step's scaled gradient)
+  float* master;   // optional fp32 master copy (nullptr: up-cast p)
+  long numel;
+  int group;
+  int p_dtype;     // 0 fp32, 1 bf16
+  int g_dtype;
+  int first;       // 1: the parameter's first step (adan.py:197-198): diff = 0, pre is written and never read
+};
+constexpr int kAdanMaxGroups = 128;
+struct AdanGroups {
+  float lr[kAdanMaxGroups];
+  float wd[kAdanMaxGroups];
+  float bc1[kAdanMaxGroups];        // 1 - b1^t with the group's step t
+  float bc2[kAdanMaxGroups];        // 1 - b2^t
+  float sqrt_bc3[kAdanMaxGroups];   // sqrt(1 - b3^t)
+  int no_prox[kAdanMaxGroups];
+  float beta1, beta2, beta3, eps;
+};
+int adan_multi_step(const void* tensors, const int* chunk_tensor, const long* chunk_off, int n_chunks,
+                    const AdanGroups& groups, const float* grad_scale, cudaStream_t stream);
+
 // ---- backward pass (backward.cu, attention_bwd.cu) ----
 long bwd_ws_floats(int dim);
 int layernorm_bwd(const void* x, int x_dtype, long ldx, const void* dy, int dy_dtype, long ld_dy, const float* gamma,

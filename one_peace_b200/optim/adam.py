@@ -16,38 +16,56 @@ import torch.optim
 from .. import _lib
 from ..fairseq_compat import FairseqOptimizer, register_optimizer
 
-_REC = np.dtype([("p", "<u8"), ("g", "<u8"), ("m", "<u8"), ("v", "<u8"), ("master", "<u8"), ("numel", "<i8"),
-                 ("group", "<i4"), ("p_dtype", "<i4"), ("g_dtype", "<i4"), ("pad", "<i4")])
-assert _REC.itemsize == 64
 _DT = {torch.float32: 0, torch.bfloat16: 1}
 _MAX_GROUPS = 128      # opb_adam_multi_step: n_groups <= 128 (include/onepeace_b200.h)
 
 
-class _Table:
-    """Device-resident tensor / chunk tables for the multi-tensor kernels; rebuilt only when a pointer moves."""
+def _ptr(t):
+    return 0 if t is None else t.data_ptr()
 
-    def __init__(self):
+
+class Layout:
+    """A record layout of the multi-tensor kernels: the numpy dtype of one record (mirroring the C struct) and
+    ``pack(entry) -> tuple`` of its field values.  Every record has a ``numel`` field."""
+
+    def __init__(self, dtype, pack):
+        self.dtype, self.pack = dtype, pack
+
+
+# AdamTensor (csrc/ops.h), also read by opb_grad_norm_clip.  entry: (p, g, m, v, master_or_None, group_index)
+ADAM_LAYOUT = Layout(
+    np.dtype([("p", "<u8"), ("g", "<u8"), ("m", "<u8"), ("v", "<u8"), ("master", "<u8"), ("numel", "<i8"),
+              ("group", "<i4"), ("p_dtype", "<i4"), ("g_dtype", "<i4"), ("pad", "<i4")]),
+    lambda e: (e[0].data_ptr(), e[1].data_ptr(), e[2].data_ptr(), e[3].data_ptr(), _ptr(e[4]), e[0].numel(), e[5],
+               _DT[e[0].dtype], _DT[e[1].dtype], 0))
+assert ADAM_LAYOUT.dtype.itemsize == 64
+
+
+class _Table:
+    """Device-resident tensor / chunk tables for the multi-tensor kernels; rebuilt only when a record changes (a moved
+    pointer, a flag)."""
+
+    def __init__(self, layout=ADAM_LAYOUT):
+        self.layout = layout
         self.key = None
         self.shape_key = None
 
     def build(self, entries, device):
-        """entries: list of (p, g, m, v, master_or_None, group_index).  The chunk tables depend on the tensor sizes only and are
-        kept while those do not change; a moved pointer (a re-allocated .grad) costs one small record upload."""
-        key = tuple((p.data_ptr(), g.data_ptr(), m.data_ptr(), v.data_ptr(), 0 if ms is None else ms.data_ptr(), gi)
-                    for p, g, m, v, ms, gi in entries)
+        """entries: what ``layout.pack`` takes (for Adam: (p, g, m, v, master_or_None, group_index)).  The chunk tables
+        depend on the tensor sizes only and are kept while those do not change; a changed record (a re-allocated .grad)
+        costs one small record upload."""
+        key = tuple(self.layout.pack(e) for e in entries)
         if key == self.key:
             return
-        rec = np.zeros(len(entries), dtype=_REC)
-        for i, (p, g, m, v, ms, gi) in enumerate(entries):
-            rec[i] = (p.data_ptr(), g.data_ptr(), m.data_ptr(), v.data_ptr(), 0 if ms is None else ms.data_ptr(),
-                      p.numel(), gi, _DT[p.dtype], _DT[g.dtype], 0)
+        rec = np.array(list(key), dtype=self.layout.dtype)
         self.tensors = torch.from_numpy(rec.view(np.uint8).copy()).to(device)
-        shape_key = (str(device),) + tuple(p.numel() for p, *_ in entries)
+        numels = [int(x) for x in rec["numel"]]
+        shape_key = (str(device),) + tuple(numels)
         if shape_key != self.shape_key:
             chunk = _lib.load().opb_adam_chunk_elems()
             ct, co = [], []
-            for i, (p, *_rest) in enumerate(entries):
-                offs = np.arange(0, p.numel(), chunk, dtype=np.int64)
+            for i, numel in enumerate(numels):
+                offs = np.arange(0, numel, chunk, dtype=np.int64)
                 ct.append(np.full(len(offs), i, dtype=np.int32))
                 co.append(offs)
             self.chunk_tensor = torch.from_numpy(np.concatenate(ct)).to(device)
@@ -171,25 +189,31 @@ class Adam(torch.optim.Optimizer):
 
     @torch.no_grad()
     def grad_norm_and_scale(self, multiply_factor=1.0, max_norm=0.0):
-        """-> fp32 device tensor [2]: {multiply_factor * ||g||_2, grad_scale}.  One deterministic two-stage reduction
-        over every gradient (replaces utils.clip_grad_norm_'s per-tensor norms + stack + norm)."""
-        entries = []
-        for gi, group in enumerate(self.param_groups):
-            for p in group["params"]:
-                if p.grad is not None:
-                    g = p.grad if p.grad.is_contiguous() else p.grad.contiguous()
-                    entries.append((p.data, g, g, g, None, gi))       # only .g / numel / dtype are read
-        if not entries:
-            return None
-        dev = entries[0][0].device
-        tab = self._norm_table        # cached: rebuilding the chunk tables (184 k chunks for the 4B vision branch) every step cost
-        tab.build(entries, dev)       # 0.3 ms of host work + three synchronous uploads, as much as the reduction itself
-        out = torch.empty(2, dtype=torch.float32, device=dev)
-        st = _lib.load().opb_grad_norm_clip(tab.tensors.data_ptr(), tab.chunk_tensor.data_ptr(), tab.chunk_off.data_ptr(),
-                                            tab.n_chunks, tab.partial.data_ptr(), float(multiply_factor), float(max_norm),
-                                            out.data_ptr(), torch.cuda.current_stream().cuda_stream)
-        _lib.check(st, "opb_grad_norm_clip")
-        return out
+        return grad_norm_and_scale(self.param_groups, self._norm_table, multiply_factor, max_norm)
+
+
+@torch.no_grad()
+def grad_norm_and_scale(param_groups, table, multiply_factor=1.0, max_norm=0.0):
+    """-> fp32 device tensor [2]: {multiply_factor * ||g||_2, grad_scale}, or None without gradients.  One deterministic
+    two-stage reduction over every gradient of ``param_groups`` (replaces utils.clip_grad_norm_'s per-tensor norms + stack
+    + norm).  ``table``: the caller's ``_Table()`` (Adam layout), kept across steps."""
+    entries = []
+    for gi, group in enumerate(param_groups):
+        for p in group["params"]:
+            if p.grad is not None:
+                g = p.grad if p.grad.is_contiguous() else p.grad.contiguous()
+                entries.append((p.data, g, g, g, None, gi))       # only .g / numel / dtype are read
+    if not entries:
+        return None
+    dev = entries[0][0].device
+    table.build(entries, dev)     # cached: rebuilding the chunk tables (184 k chunks for the 4B vision branch) every step cost
+    #                               0.3 ms of host work + three synchronous uploads, as much as the reduction itself
+    out = torch.empty(2, dtype=torch.float32, device=dev)
+    st = _lib.load().opb_grad_norm_clip(table.tensors.data_ptr(), table.chunk_tensor.data_ptr(), table.chunk_off.data_ptr(),
+                                        table.n_chunks, table.partial.data_ptr(), float(multiply_factor), float(max_norm),
+                                        out.data_ptr(), torch.cuda.current_stream().cuda_stream)
+    _lib.check(st, "opb_grad_norm_clip")
+    return out
 
 
 @register_optimizer("adjust_adam")
