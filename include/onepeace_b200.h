@@ -236,12 +236,14 @@ int opb_transpose_bf16(const void* in, int64_t ld_in, void* out, int rows, int c
  * fp32 [rows, d] -> bf16 [rows, 3d] split x = hi + lo: side 0 -> [hi|hi|lo] (local operand), side 1 -> [hi|lo|hi]
  * (gathered operand).  One K = 3d GEMM then gives hi.hi + hi.lo + lo.hi, i.e. logits accurate to ~2^-16 — the similarity
  * matrices of criterions/image_text_retrieval_loss.py:95-96 and metrics/recall.py:33 are fp32 products in the reference.
+ * 1 <= count <= 4 tensors of the same d in one launch; xs / outs / rows / sides: HOST arrays of count.
  */
-int opb_split_bf16x3(const float* x, void* out, int64_t rows, int d, int side, void* stream);
+int opb_split_bf16x3(const float* const* xs, void* const* outs, const int64_t* rows, const int* sides, int count, int d,
+                     void* stream);
 
 /*
- * Cross-modal InfoNCE, one direction (criterions/image_text_retrieval_loss.py:91-112, :16-26; pretrain twin
- * image_text_pretrain_loss.py:164-185).  a_local bf16 [b,k] (this rank's rows), b_all bf16 [n,k] (all ranks'
+ * Cross-modal InfoNCE (criterions/image_text_retrieval_loss.py:91-112, :16-26; pretrain twin
+ * image_text_pretrain_loss.py:164-185).  One direction: a_local bf16 [b,k] (this rank's rows), b_all bf16 [n,k] (all ranks'
  * rows of the other modality in rank-major order, detached); k = d for plain bf16 operands or 3d for the
  * opb_split_bf16x3 layout; scale = device scalar exp(clamp(logit_scale)).
  * Targets: row i -> column i + target_offset (target_offset = rank * b).
@@ -249,40 +251,29 @@ int opb_split_bf16x3(const float* x, void* out, int64_t rows, int d, int side, v
  * (-inf logits, zero gradient).  coef (0 = 1 / (2 b)): weight of a row's loss in the gradient.  These two serve the
  * single-direction DCL loss (image_text_pretrain_loss.py:187-208: masked student rows vs the local batch's teacher rows,
  * mean over rows -> coef = 1 / b), which is the same tiled similarity + log-softmax as one InfoNCE direction.
- *   opb_infonce_ws_floats : size (floats) of the partial workspace `ws` for opb_infonce_rows
- *   opb_infonce_rows      : row_lse / row_loss (label-smoothed NLL per row) / row_argmax, all [b]
- *   opb_infonce_reduce    : out3 = {(mean(loss_a) + mean(loss_b)) / 2, #correct a->b, #correct b->a}
- *   opb_infonce_grad      : grad_a fp32 [b,d] = d(loss)/d(a_local) (local rows only; no gradient to b_all, :30-38);
- *                           bT_all bf16 [d,n] = b_all transposed, or NULL: b_all is then read in place as the MN-major operand
- *                           of the G . B_all product (no transposed copy); g_ws bf16 [b,n] scratch; ws_gz [ceil(n/256), b]
- *   opb_infonce_dscale    : out[0] = d(loss)/d(logit_scale) from the two directions' ws_gz
+ *   opb_infonce_ws_floats     size (floats) of the partial workspace `ws` of one direction
+ *   opb_infonce_lse_gemm      the LSE_PARTIAL GEMM of one direction: per-tile row partials into ws
+ *   opb_infonce_merge_reduce  merges one or both directions' partials (ws_b = row_lse_b = NULL: one direction; dirs = 1 or 2)
+ *                             into row_lse [b] per direction (needed by opb_infonce_grad) and writes out3 = {sum of the
+ *                             dirs * b row losses / (dirs * b), #correct a->b, #correct b->a (0 for one direction)} in one
+ *                             launch: the last block to finish performs the fixed-order reduction.  loss_ab fp32 [dirs * b]
+ *                             (label-smoothed NLL per row) and argmax_ab int32 [dirs * b] hold direction a's rows, then b's;
+ *                             ticket = one uint32 that must be zero on entry and is left at zero.
+ *   opb_infonce_grad          grad_a fp32 [b,d] = d(loss)/d(a_local) (local rows only; no gradient to b_all, :30-38);
+ *                             b_all is read in place as the MN-major operand of the G . B_all product (no transposed copy);
+ *                             g_ws bf16 [b,n] scratch; ws_gz [ceil(n/256), b]
+ *   opb_infonce_dscale        out[0] = d(loss)/d(logit_scale) from the two directions' ws_gz
  */
 int64_t opb_infonce_ws_floats(int b, int n);
-int opb_infonce_rows(const void* a_local, const void* b_all, const float* scale, int b, int n, int d,
-                     int target_offset, float label_smoothing, float* ws, float* row_lse, float* row_loss,
-                     int* row_argmax, int n_valid, void* stream);
-int opb_infonce_reduce(const float* loss_a, const float* loss_b, const int* argmax_a, const int* argmax_b, int b,
-                       int target_offset, float* out3, void* stream);
-int opb_infonce_grad(const void* a_local, const void* b_all, const void* bT_all, const float* scale,
-                     const float* row_lse, int b, int n, int d, int k_logits, int target_offset,
-                     float label_smoothing, void* g_ws, float* ws_gz, float* grad_a, int n_valid, float coef,
-                     void* stream);
-int opb_infonce_dscale(const float* ws_gz_a, const float* ws_gz_b, int b, int n, float* out, void* stream);
-
-/* The two-direction step with fewer launches (9 instead of 14; same arithmetic as the entries above):
- *   opb_split_bf16x3_x4       the four operand splits (a_local, b_local: side 0; a_all, b_all: side 1) in one launch;
- *                             xs / outs / rows / sides: HOST arrays of 4
- *   opb_infonce_lse_gemm      the LSE_PARTIAL GEMM of one direction (what opb_infonce_rows runs before its merge kernel)
- *   opb_infonce_merge_reduce  merges both directions' partials (row_lse_a / row_lse_b out, needed by opb_infonce_grad) and writes
- *                             out3 as opb_infonce_reduce does, in one launch: the last block to finish performs the fixed-order
- *                             reduction.  Scratch: loss_ab fp32 [2 b], argmax_ab int32 [2 b], ticket = one uint32 that must be
- *                             zero on entry and is left at zero. */
-int opb_split_bf16x3_x4(const float* const* xs, void* const* outs, const int64_t* rows, const int* sides, int d, void* stream);
 int opb_infonce_lse_gemm(const void* a_local, const void* b_all, const float* scale, int b, int n, int d, int target_offset,
                          float* ws, int n_valid, void* stream);
 int opb_infonce_merge_reduce(const float* ws_a, const float* ws_b, int b, int n, int n_valid, float label_smoothing,
                              int target_offset, float* row_lse_a, float* row_lse_b, float* loss_ab, int* argmax_ab, float* out3,
                              uint32_t* ticket, void* stream);
+int opb_infonce_grad(const void* a_local, const void* b_all, const float* scale, const float* row_lse, int b, int n, int d,
+                     int k_logits, int target_offset, float label_smoothing, void* g_ws, float* ws_gz, float* grad_a,
+                     int n_valid, float coef, void* stream);
+int opb_infonce_dscale(const float* ws_gz_a, const float* ws_gz_b, int b, int n, float* out, void* stream);
 
 /*
  * Fused multi-tensor Adam (optim/adam.py:173-253 python form; optional fp32 master as optim/adam_fused.py:45-50)

@@ -43,15 +43,11 @@ SIGNATURES = {
     "opb_l2_normalize_rows": (c_int, [c_void_p, c_int64, c_void_p, c_void_p, c_int, c_int, c_void_p]),
     "opb_zero_padded_rows": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p]),
     "opb_transpose_bf16": (c_int, [c_void_p, c_int64, c_void_p, c_int, c_int, c_void_p]),
-    "opb_split_bf16x3": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int, c_void_p]),
+    "opb_split_bf16x3": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p]),
     "opb_infonce_ws_floats": (c_int64, [c_int, c_int]),
-    "opb_infonce_rows": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p, c_void_p,
-                                 c_void_p, c_void_p, c_int, c_void_p]),
-    "opb_infonce_reduce": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p]),
-    "opb_infonce_grad": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int,
+    "opb_infonce_grad": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int,
                                  c_float, c_void_p, c_void_p, c_void_p, c_int, c_float, c_void_p]),
     "opb_infonce_dscale": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p]),
-    "opb_split_bf16x3_x4": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p]),
     "opb_infonce_lse_gemm": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int, c_void_p]),
     "opb_infonce_merge_reduce": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_float, c_int, c_void_p, c_void_p, c_void_p,
                                          c_void_p, c_void_p, c_void_p, c_void_p]),

@@ -188,17 +188,15 @@ class DclLossFn(torch.autograd.Function):
         s_rows = K.row_gather(student.detach().float().contiguous(), stu_idx)            # fp32 [n_m, d]
         t_rows = K.row_gather(teacher.detach().float().contiguous(), tidx.contiguous())  # fp32 [n8, d], zero rows past n_t
         s_n, t_n = K.l2_normalize_rows(s_rows), K.l2_normalize_rows(t_rows)              # F.normalize(x.float(), dim=1)
-        a3, b3 = K.split_bf16x3(s_n, 0), K.split_bf16x3(t_n, 1)
+        a3, b3 = K.split_bf16x3([s_n, t_n], [0, 1])
         sc = torch.full((1,), float(scale), dtype=torch.float32, device=dev)
-        lse, row_loss, am = K.infonce_rows(a3, b3, sc, 0, eps, n_valid=n_t)
-        zeros = torch.zeros_like(row_loss)
-        out = K.infonce_reduce(row_loss, zeros, am, am, 0)                               # out[0] = mean(row_loss) / 2
+        (lse,), out = K.infonce_forward([(a3, b3)], sc, 0, eps, n_valid=n_t)           # out[0] = mean(row_loss)
         if student.requires_grad:
-            grad_n, _ = K.infonce_grad(a3, b3, None, sc, lse, 0, eps, n_valid=n_t, coef=1.0 / n_m, d=d)
+            grad_n, _ = K.infonce_grad(a3, b3, sc, lse, 0, eps, d, n_valid=n_t, coef=1.0 / n_m)
             dx16, dx32 = K.l2_normalize_bwd(s_rows, grad_n, want_f32=True)
             ctx.save_for_backward(dx32, stu_idx)
         ctx.meta = (student.shape, student.dtype)
-        return out[0] * 2.0
+        return out[0]
 
     @staticmethod
     def backward(ctx, g_loss):

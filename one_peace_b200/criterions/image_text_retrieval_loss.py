@@ -39,16 +39,16 @@ class _InfoNCE(torch.autograd.Function):
         if n_cls % 8:                 # the GEMM wants N % 8 == 0: zero rows, ignored through n_valid (tiny global batches)
             padr = torch.zeros((-n_cls) % 8, d, dtype=torch.float32, device=fa.device)
             fa, fb = torch.cat([fa, padr]), torch.cat([fb, padr])
-        a3, b3, a_all3, b_all3 = K.split_bf16x3_x4([f32(a_local), f32(b_local), fa, fb], [0, 0, 1, 1])
+        a3, b3, a_all3, b_all3 = K.split_bf16x3([f32(a_local), f32(b_local), fa, fb], [0, 0, 1, 1])
         s = scale.detach().to(torch.float32).reshape(1).contiguous()
         bsz, n = a3.shape[0], a_all3.shape[0]
         nv = n_cls if n_cls != n else 0
         off = bsz * rank
         # two LSE GEMMs + ONE merge / reduce kernel for both directions (the last block to finish does the fixed-order reduction)
-        lse_a, lse_b, out = K.infonce_forward2(a3, b3, a_all3, b_all3, s, off, eps, n_valid=nv)
+        (lse_a, lse_b), out = K.infonce_forward([(a3, b_all3), (b3, a_all3)], s, off, eps, n_valid=nv)
         if a_local.requires_grad or b_local.requires_grad or scale.requires_grad:
-            ga, ws_a = K.infonce_grad(a3, b_all3, None, s, lse_a, off, eps, n_valid=nv, d=d)      # G . B_all reads B_all MN-major
-            gb, ws_b = K.infonce_grad(b3, a_all3, None, s, lse_b, off, eps, n_valid=nv, d=d)
+            ga, ws_a = K.infonce_grad(a3, b_all3, s, lse_a, off, eps, d, n_valid=nv)      # G . B_all reads B_all MN-major
+            gb, ws_b = K.infonce_grad(b3, a_all3, s, lse_b, off, eps, d, n_valid=nv)
             dlogit = K.infonce_dscale(ws_a, ws_b, bsz, n)        # d loss / d log(scale)
             ctx.save_for_backward(ga, gb, dlogit, s)
         ctx.dtypes = (a_local.dtype, b_local.dtype, scale.dtype)

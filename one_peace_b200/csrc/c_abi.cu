@@ -9,7 +9,7 @@
 
 extern "C" {
 
-int opb_abi_version(void) { return 2; }
+int opb_abi_version(void) { return 3; }
 
 const char* opb_status_string(int status) {
   switch (status) {
@@ -173,19 +173,13 @@ int opb_transpose_bf16(const void* in, int64_t ld_in, void* out, int rows, int c
   return opb::transpose_bf16(in, ld_in, out, rows, cols, static_cast<cudaStream_t>(stream));
 }
 
-int opb_split_bf16x3(const float* x, void* out, int64_t rows, int d, int side, void* stream) {
-  if (!x || !out) return OPB_ERR_INVALID;
-  return opb::split_bf16x3(x, out, rows, d, side, static_cast<cudaStream_t>(stream));
+int opb_split_bf16x3(const float* const* xs, void* const* outs, const int64_t* rows, const int* sides, int count, int d,
+                     void* stream) {
+  if (!xs || !outs || !rows || !sides) return OPB_ERR_INVALID;
+  return opb::split_bf16x3(xs, outs, rows, sides, count, d, static_cast<cudaStream_t>(stream));
 }
 
 int64_t opb_infonce_ws_floats(int b, int n) { return opb::infonce_ws_floats(b, n); }
-
-int opb_split_bf16x3_x4(const float* const* xs, void* const* outs, const int64_t* rows, const int* sides, int d, void* stream) {
-  if (!xs || !outs || !rows || !sides) return OPB_ERR_INVALID;
-  long r[4];
-  for (int t = 0; t < 4; ++t) r[t] = static_cast<long>(rows[t]);
-  return opb::split_bf16x3_x4(xs, outs, r, sides, d, static_cast<cudaStream_t>(stream));
-}
 
 int opb_infonce_lse_gemm(const void* a_local, const void* b_all, const float* scale, int b, int n, int d, int target_offset,
                          float* ws, int n_valid, void* stream) {
@@ -196,32 +190,16 @@ int opb_infonce_lse_gemm(const void* a_local, const void* b_all, const float* sc
 int opb_infonce_merge_reduce(const float* ws_a, const float* ws_b, int b, int n, int n_valid, float label_smoothing,
                              int target_offset, float* row_lse_a, float* row_lse_b, float* loss_ab, int* argmax_ab, float* out3,
                              uint32_t* ticket, void* stream) {
-  if (!ws_a || !ws_b || !row_lse_a || !row_lse_b || !loss_ab || !argmax_ab || !out3 || !ticket) return OPB_ERR_INVALID;
+  if (!ws_a || !row_lse_a || !loss_ab || !argmax_ab || !out3 || !ticket) return OPB_ERR_INVALID;
   return opb::infonce_merge_reduce(ws_a, ws_b, b, n, n_valid, label_smoothing, target_offset, row_lse_a, row_lse_b, loss_ab,
                                    argmax_ab, out3, ticket, static_cast<cudaStream_t>(stream));
 }
 
-int opb_infonce_rows(const void* a_local, const void* b_all, const float* scale, int b, int n, int d,
-                     int target_offset, float label_smoothing, float* ws, float* row_lse, float* row_loss,
-                     int* row_argmax, int n_valid, void* stream) {
-  if (!a_local || !b_all || !scale || !ws || !row_lse || !row_loss || !row_argmax) return OPB_ERR_INVALID;
-  return opb::infonce_rows(a_local, b_all, scale, b, n, d, target_offset, label_smoothing, ws, row_lse, row_loss,
-                           row_argmax, n_valid, static_cast<cudaStream_t>(stream));
-}
-
-int opb_infonce_reduce(const float* loss_a, const float* loss_b, const int* argmax_a, const int* argmax_b, int b,
-                       int target_offset, float* out3, void* stream) {
-  if (!loss_a || !loss_b || !argmax_a || !argmax_b || !out3 || b <= 0) return OPB_ERR_INVALID;
-  return opb::infonce_reduce(loss_a, loss_b, argmax_a, argmax_b, b, target_offset, out3,
-                             static_cast<cudaStream_t>(stream));
-}
-
-int opb_infonce_grad(const void* a_local, const void* b_all, const void* bT_all, const float* scale,
-                     const float* row_lse, int b, int n, int d, int k_logits, int target_offset,
-                     float label_smoothing, void* g_ws, float* ws_gz, float* grad_a, int n_valid, float coef,
-                     void* stream) {
+int opb_infonce_grad(const void* a_local, const void* b_all, const float* scale, const float* row_lse, int b, int n, int d,
+                     int k_logits, int target_offset, float label_smoothing, void* g_ws, float* ws_gz, float* grad_a,
+                     int n_valid, float coef, void* stream) {
   if (!a_local || !b_all || !scale || !row_lse || !g_ws || !ws_gz || !grad_a) return OPB_ERR_INVALID;
-  return opb::infonce_grad(a_local, b_all, bT_all, scale, row_lse, b, n, d, k_logits, target_offset, label_smoothing,
+  return opb::infonce_grad(a_local, b_all, scale, row_lse, b, n, d, k_logits, target_offset, label_smoothing,
                            g_ws, ws_gz, grad_a, n_valid, coef, static_cast<cudaStream_t>(stream));
 }
 

@@ -13,62 +13,6 @@
 
 namespace opb {
 
-// merge the per-tile partials of one direction: lse, loss and arg-max per row
-__global__ void infonce_merge_kernel(const float* __restrict__ ws, int n_tiles, int b, int n, float eps,
-                                     float* __restrict__ row_lse, float* __restrict__ row_loss,
-                                     int* __restrict__ row_argmax) {
-  const int row = blockIdx.x * blockDim.x + threadIdx.x;
-  if (row >= b) return;
-  float m = -INFINITY;
-  for (int t = 0; t < n_tiles; ++t) m = fmaxf(m, ws[(static_cast<long>(t) * b + row) * 8]);
-  float s = 0.f, zsum = 0.f, best = -INFINITY, ztgt = 0.f;
-  int best_idx = 0;
-  for (int t = 0; t < n_tiles; ++t) {
-    const float* w = ws + (static_cast<long>(t) * b + row) * 8;
-    const float4 p0 = *reinterpret_cast<const float4*>(w);
-    const float4 p1 = *reinterpret_cast<const float4*>(w + 4);
-    s += p0.y * __expf(p0.x - m);
-    zsum += p0.z;
-    if (p0.w > best) { best = p0.w; best_idx = __float_as_int(p1.x); }   // strict >: first maximum wins (torch.argmax)
-    if (p1.z != 0.f) ztgt = p1.y;
-  }
-  const float lse = m + logf(s);
-  const float nll = lse - ztgt;
-  float loss = nll;
-  if (eps != 0.f) {
-    const float eps_i = eps / (n - 1);
-    loss = (1.f - eps - eps_i) * nll + eps_i * (n * lse - zsum);
-  }
-  row_lse[row] = lse;
-  row_loss[row] = loss;
-  row_argmax[row] = best_idx;
-}
-
-// out[0] = (mean(loss_a) + mean(loss_b)) / 2, out[1] = #(argmax_a == target), out[2] = #(argmax_b == target)
-// single block, fixed summation order (deterministic across ranks / runs)
-__global__ void infonce_reduce_kernel(const float* __restrict__ loss_a, const float* __restrict__ loss_b,
-                                      const int* __restrict__ am_a, const int* __restrict__ am_b, int b,
-                                      int target_offset, float* __restrict__ out) {
-  __shared__ float red[3][32];
-  float la = 0.f, ca = 0.f, cb = 0.f;
-  for (int i = threadIdx.x; i < b; i += blockDim.x) {
-    la += loss_a[i] + loss_b[i];
-    ca += (am_a[i] == i + target_offset) ? 1.f : 0.f;
-    cb += (am_b[i] == i + target_offset) ? 1.f : 0.f;
-  }
-  la = warp_sum(la); ca = warp_sum(ca); cb = warp_sum(cb);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (lane == 0) { red[0][warp] = la; red[1][warp] = ca; red[2][warp] = cb; }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    float t0 = 0.f, t1 = 0.f, t2 = 0.f;
-    for (int w = 0; w < (blockDim.x >> 5); ++w) { t0 += red[0][w]; t1 += red[1][w]; t2 += red[2][w]; }
-    out[0] = t0 / (2.f * b);
-    out[1] = t1;
-    out[2] = t2;
-  }
-}
-
 // d(loss)/d(logit_scale) = coef * sum_ij G_ij z_ij over both directions (ws_a / ws_b: [n_tiles, b] partials)
 __global__ void infonce_dscale_kernel(const float* __restrict__ ws_a, const float* __restrict__ ws_b, long count,
                                       float coef, float* __restrict__ out) {
@@ -154,41 +98,15 @@ int transpose_bf16(const void* in, long ld_in, void* out, int rows, int cols, cu
 // side 0 (the local operand): [hi | hi | lo];  side 1 (the gathered operand): [hi | lo | hi], so that one K = 3d
 // wgmma GEMM yields hi.hi + hi.lo + lo.hi — the logits to ~2^-16 relative instead of bf16's 2^-9, which is what
 // keeps the loss within 1e-3 of the fp32 oracle at small d / large logit_scale.
-__global__ void split_bf16x3_kernel(const float* __restrict__ x, __nv_bfloat16* __restrict__ out, long total, int d,
-                                    int side) {
-  for (long i = blockIdx.x * static_cast<long>(blockDim.x) + threadIdx.x; i < total;
-       i += static_cast<long>(gridDim.x) * blockDim.x) {
-    const long r = i / d;
-    const int c = i % d;
-    const float v = x[i];
-    const __nv_bfloat16 hi = __float2bfloat16(v);
-    const __nv_bfloat16 lo = __float2bfloat16(v - __bfloat162float(hi));
-    __nv_bfloat16* o = out + r * 3L * d + c;
-    o[0] = hi;
-    o[d] = side == 0 ? hi : lo;
-    o[2L * d] = side == 0 ? lo : hi;
-  }
-}
-
-int split_bf16x3(const float* x, void* out, long rows, int d, int side, cudaStream_t stream) {
-  if (rows <= 0 || d <= 0 || (side != 0 && side != 1)) return OPB_ERR_INVALID;
-  const long total = rows * d;
-  long blocks = (total + 255) / 256;
-  if (blocks > 132L * 16) blocks = 132L * 16;
-  split_bf16x3_kernel<<<static_cast<unsigned>(blocks), 256, 0, stream>>>(x, reinterpret_cast<__nv_bfloat16*>(out), total,
-                                                                       d, side);
-  return cudaGetLastError() == cudaSuccess ? OPB_OK : OPB_ERR_CUDA;
-}
-
-// the four operand splits of one InfoNCE step (a_local, b_local: side 0; a_all, b_all: side 1) in ONE launch: blockIdx.y selects
-// the tensor (round 2: the head was 14 launches for 0.36 ms of work)
-struct Split4 {
+// Up to four tensors in ONE launch (the operands of one InfoNCE step: a_local, b_local side 0; a_all, b_all side 1):
+// blockIdx.y selects the tensor.
+struct SplitArgs {
   const float* x[4];
   __nv_bfloat16* out[4];
   long total[4];
   int side[4];
 };
-__global__ void split_bf16x3_x4_kernel(const Split4 sp, int d) {
+__global__ void split_bf16x3_kernel(const SplitArgs sp, int d) {
   const int t = blockIdx.y;
   const float* __restrict__ x = sp.x[t];
   __nv_bfloat16* __restrict__ out = sp.out[t];
@@ -208,30 +126,33 @@ __global__ void split_bf16x3_x4_kernel(const Split4 sp, int d) {
   }
 }
 
-int split_bf16x3_x4(const float* const* xs, void* const* outs, const long* rows, const int* sides, int d, cudaStream_t stream) {
-  if (d <= 0) return OPB_ERR_INVALID;
-  Split4 sp;
+int split_bf16x3(const float* const* xs, void* const* outs, const int64_t* rows, const int* sides, int count, int d,
+                 cudaStream_t stream) {
+  if (count < 1 || count > 4 || d <= 0) return OPB_ERR_INVALID;
+  SplitArgs sp;
   long mx = 0;
-  for (int t = 0; t < 4; ++t) {
+  for (int t = 0; t < count; ++t) {
     if (xs[t] == nullptr || outs[t] == nullptr || rows[t] <= 0 || (sides[t] != 0 && sides[t] != 1)) return OPB_ERR_INVALID;
     sp.x[t] = xs[t]; sp.out[t] = reinterpret_cast<__nv_bfloat16*>(outs[t]); sp.total[t] = rows[t] * d; sp.side[t] = sides[t];
     if (sp.total[t] > mx) mx = sp.total[t];
   }
   long blocks = (mx + 255) / 256;
-  if (blocks > 132L * 4) blocks = 132L * 4;
-  split_bf16x3_x4_kernel<<<dim3(static_cast<unsigned>(blocks), 4), 256, 0, stream>>>(sp, d);
+  if (blocks > 132L * 16 / count) blocks = 132L * 16 / count;      // at most 16 blocks per SM over all tensors
+  split_bf16x3_kernel<<<dim3(static_cast<unsigned>(blocks), count), 256, 0, stream>>>(sp, d);
   return cudaGetLastError() == cudaSuccess ? OPB_OK : OPB_ERR_CUDA;
 }
 
-// merge of BOTH directions' per-tile partials + the step's scalar outputs in one launch.  blockIdx.y = direction; every block
-// merges 128 rows (as infonce_merge_kernel) and takes a ticket; the LAST block to finish sums all 2 b row losses / hit flags in a
-// fixed order (the result does not depend on which block that is) and resets the ticket counter for the next call.
+// merge of one or both directions' per-tile partials + the step's scalar outputs in one launch.  blockIdx.y = direction
+// (gridDim.y = 1 or 2); every block merges 128 rows and takes a ticket; the LAST block to finish sums all gridDim.y * b row
+// losses / hit flags in a fixed order (the result does not depend on which block that is) and resets the ticket counter for
+// the next call.
 __global__ void __launch_bounds__(128)
-infonce_merge2_reduce_kernel(const float* __restrict__ ws_a, const float* __restrict__ ws_b, int n_tiles, int b, int n, float eps,
-                             int target_offset, float* __restrict__ lse_a, float* __restrict__ lse_b, float* __restrict__ loss_ab,
-                             int* __restrict__ am_ab, float* __restrict__ out3, unsigned int* __restrict__ ticket) {
+infonce_merge_reduce_kernel(const float* __restrict__ ws_a, const float* __restrict__ ws_b, int n_tiles, int b, int n, float eps,
+                            int target_offset, float* __restrict__ lse_a, float* __restrict__ lse_b, float* __restrict__ loss_ab,
+                            int* __restrict__ am_ab, float* __restrict__ out3, unsigned int* __restrict__ ticket) {
   __shared__ float red[3][4];
   __shared__ bool last;
+  const int dirs = gridDim.y;
   const int dir = blockIdx.y;
   const float* __restrict__ ws = dir == 0 ? ws_a : ws_b;
   float* __restrict__ row_lse = dir == 0 ? lse_a : lse_b;
@@ -247,7 +168,7 @@ infonce_merge2_reduce_kernel(const float* __restrict__ ws_a, const float* __rest
       const float4 p1 = *reinterpret_cast<const float4*>(w + 4);
       s += p0.y * __expf(p0.x - m);
       zsum += p0.z;
-      if (p0.w > best) { best = p0.w; best_idx = __float_as_int(p1.x); }
+      if (p0.w > best) { best = p0.w; best_idx = __float_as_int(p1.x); }   // strict >: first maximum wins (torch.argmax)
       if (p1.z != 0.f) ztgt = p1.y;
     }
     const float lse = m + logf(s);
@@ -269,9 +190,13 @@ infonce_merge2_reduce_kernel(const float* __restrict__ ws_a, const float* __rest
   __threadfence();
   float la = 0.f, ca = 0.f, cb = 0.f;
   for (int i = threadIdx.x; i < b; i += blockDim.x) {
-    la += __ldcg(loss_ab + i) + __ldcg(loss_ab + b + i);
+    float l = __ldcg(loss_ab + i);
     ca += (__ldcg(am_ab + i) == i + target_offset) ? 1.f : 0.f;
-    cb += (__ldcg(am_ab + b + i) == i + target_offset) ? 1.f : 0.f;
+    if (dirs == 2) {
+      l += __ldcg(loss_ab + b + i);
+      cb += (__ldcg(am_ab + b + i) == i + target_offset) ? 1.f : 0.f;
+    }
+    la += l;
   }
   la = warp_sum(la); ca = warp_sum(ca); cb = warp_sum(cb);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -280,7 +205,7 @@ infonce_merge2_reduce_kernel(const float* __restrict__ ws_a, const float* __rest
   if (threadIdx.x == 0) {
     float t0 = 0.f, t1 = 0.f, t2 = 0.f;
     for (int w = 0; w < 4; ++w) { t0 += red[0][w]; t1 += red[1][w]; t2 += red[2][w]; }
-    out3[0] = t0 / (2.f * b);
+    out3[0] = t0 / (static_cast<float>(dirs) * b);
     out3[1] = t1;
     out3[2] = t2;
     *ticket = 0u;
@@ -291,30 +216,12 @@ static int n_tiles_of(int n) { return (n + 255) / 256; }
 
 long infonce_ws_floats(int b, int n) { return static_cast<long>(n_tiles_of(n)) * b * 8; }
 
-// forward for one direction: row_lse / row_loss / row_argmax
-int infonce_rows(const void* a_local, const void* b_all, const float* scale, int b, int n, int d, int target_offset,
-                 float eps, float* ws, float* row_lse, float* row_loss, int* row_argmax, int n_valid, cudaStream_t stream) {
-  if (b <= 0 || n <= 0 || d <= 0 || d % 8 != 0 || n % 8 != 0 || n_valid < 0 || n_valid > n) return OPB_ERR_INVALID;
-  const int n_cls = n_valid > 0 ? n_valid : n;
-  GemmEpilogue ep;
-  ep.out = ws;            // unused by this epilogue but must be non-null for the generic checks
-  ep.scale_ptr = scale;
-  ep.ws = ws;
-  ep.target_offset = target_offset;
-  ep.n_valid = n_valid;
-  int rc = gemm_bf16(a_local, d, b_all, d, b, n, d, EPI_LSE_PARTIAL, ep, 0, stream);
-  if (rc != OPB_OK) return rc;
-  infonce_merge_kernel<<<(b + 127) / 128, 128, 0, stream>>>(ws, n_tiles_of(n), b, n_cls, eps, row_lse, row_loss,
-                                                            row_argmax);
-  return cudaGetLastError() == cudaSuccess ? OPB_OK : OPB_ERR_CUDA;
-}
-
-// LSE_PARTIAL GEMM of one direction only (the merge runs later, for both directions at once: infonce_merge_reduce)
+// LSE_PARTIAL GEMM of one direction (the merge runs later, for every direction at once: infonce_merge_reduce)
 int infonce_lse_gemm(const void* a_local, const void* b_all, const float* scale, int b, int n, int d, int target_offset, float* ws,
                      int n_valid, cudaStream_t stream) {
   if (b <= 0 || n <= 0 || d <= 0 || d % 8 != 0 || n % 8 != 0 || n_valid < 0 || n_valid > n) return OPB_ERR_INVALID;
   GemmEpilogue ep;
-  ep.out = ws;
+  ep.out = ws;            // unused by this epilogue but must be non-null for the generic checks
   ep.scale_ptr = scale;
   ep.ws = ws;
   ep.target_offset = target_offset;
@@ -322,26 +229,22 @@ int infonce_lse_gemm(const void* a_local, const void* b_all, const float* scale,
   return gemm_bf16(a_local, d, b_all, d, b, n, d, EPI_LSE_PARTIAL, ep, 0, stream);
 }
 
-// scratch: loss_ab fp32 [2 b], am_ab int32 [2 b], ticket: one zero-initialised uint32 (left at zero)
+// ws_b == lse_b == nullptr: one direction.  scratch: loss_ab fp32 [dirs b], am_ab int32 [dirs b], ticket: one zero-initialised
+// uint32 (left at zero)
 int infonce_merge_reduce(const float* ws_a, const float* ws_b, int b, int n, int n_valid, float eps, int target_offset, float* lse_a,
                          float* lse_b, float* loss_ab, int* am_ab, float* out3, unsigned int* ticket, cudaStream_t stream) {
-  if (b <= 0 || n <= 0 || n_valid < 0 || n_valid > n) return OPB_ERR_INVALID;
+  if (b <= 0 || n <= 0 || n_valid < 0 || n_valid > n || (ws_b == nullptr) != (lse_b == nullptr)) return OPB_ERR_INVALID;
   const int n_cls = n_valid > 0 ? n_valid : n;
-  infonce_merge2_reduce_kernel<<<dim3((b + 127) / 128, 2), 128, 0, stream>>>(ws_a, ws_b, n_tiles_of(n), b, n_cls, eps, target_offset,
-                                                                             lse_a, lse_b, loss_ab, am_ab, out3, ticket);
-  return cudaGetLastError() == cudaSuccess ? OPB_OK : OPB_ERR_CUDA;
-}
-
-int infonce_reduce(const float* loss_a, const float* loss_b, const int* am_a, const int* am_b, int b,
-                   int target_offset, float* out3, cudaStream_t stream) {
-  infonce_reduce_kernel<<<1, 1024, 0, stream>>>(loss_a, loss_b, am_a, am_b, b, target_offset, out3);
+  const int dirs = ws_b != nullptr ? 2 : 1;
+  infonce_merge_reduce_kernel<<<dim3((b + 127) / 128, dirs), 128, 0, stream>>>(ws_a, ws_b, n_tiles_of(n), b, n_cls, eps, target_offset,
+                                                                                lse_a, lse_b, loss_ab, am_ab, out3, ticket);
   return cudaGetLastError() == cudaSuccess ? OPB_OK : OPB_ERR_CUDA;
 }
 
 // backward for one direction: grad_a fp32 [b, d] = (s / 2b) G B_all ; ws_gz [n_tiles, b] row partials of sum G z
-int infonce_grad(const void* a_local, const void* b_all, const void* bT_all, const float* scale,
-                 const float* row_lse, int b, int n, int d, int k_logits, int target_offset, float eps, void* g_ws,
-                 float* ws_gz, float* grad_a, int n_valid, float coef, cudaStream_t stream) {
+int infonce_grad(const void* a_local, const void* b_all, const float* scale, const float* row_lse, int b, int n, int d,
+                 int k_logits, int target_offset, float eps, void* g_ws, float* ws_gz, float* grad_a, int n_valid, float coef,
+                 cudaStream_t stream) {
   if (b <= 0 || n <= 0 || d <= 0 || d % 8 != 0 || n % 8 != 0 || k_logits % 8 != 0 || n_valid < 0 || n_valid > n)
     return OPB_ERR_INVALID;
   const int n_cls = n_valid > 0 ? n_valid : n;
@@ -362,8 +265,7 @@ int infonce_grad(const void* a_local, const void* b_all, const void* bT_all, con
   e2.out = grad_a;
   e2.ldo = d;
   // grad_a = G . B_all: a contraction over the n gathered rows.  B_all ([n, k_logits], its first d columns = the bf16 "hi" part)
-  // is the MN-major B operand as it stands; the explicit transpose (bT_all) is kept for A/B runs only.
-  if (bT_all != nullptr) return gemm_bf16(g_ws, n, bT_all, n, b, d, n, EPI_STORE_F32, e2, 0, stream);
+  // is the MN-major B operand as it stands, so no transposed copy is needed.
   return gemm_bf16_t(g_ws, n, 0, b_all, k_logits, 1, b, d, n, EPI_STORE_F32, e2, 0, stream);
 }
 

@@ -55,20 +55,16 @@ int l2_normalize_rows(const float* x, long ldx, float* y, void* y_bf16, int rows
 int zero_padded_rows(float* x, const uint8_t* pad_mask, int rows, int D, cudaStream_t stream);
 
 int transpose_bf16(const void* in, long ld_in, void* out, int rows, int cols, cudaStream_t stream);
-int split_bf16x3(const float* x, void* out, long rows, int d, int side, cudaStream_t stream);
-int split_bf16x3_x4(const float* const* xs, void* const* outs, const long* rows, const int* sides, int d, cudaStream_t stream);
+int split_bf16x3(const float* const* xs, void* const* outs, const int64_t* rows, const int* sides, int count, int d,
+                 cudaStream_t stream);
 int infonce_lse_gemm(const void* a_local, const void* b_all, const float* scale, int b, int n, int d, int target_offset, float* ws,
                      int n_valid, cudaStream_t stream);
 int infonce_merge_reduce(const float* ws_a, const float* ws_b, int b, int n, int n_valid, float eps, int target_offset, float* lse_a,
                          float* lse_b, float* loss_ab, int* am_ab, float* out3, unsigned int* ticket, cudaStream_t stream);
 long infonce_ws_floats(int b, int n);
-int infonce_rows(const void* a_local, const void* b_all, const float* scale, int b, int n, int d, int target_offset,
-                 float eps, float* ws, float* row_lse, float* row_loss, int* row_argmax, int n_valid, cudaStream_t stream);
-int infonce_reduce(const float* loss_a, const float* loss_b, const int* am_a, const int* am_b, int b,
-                   int target_offset, float* out3, cudaStream_t stream);
-int infonce_grad(const void* a_local, const void* b_all, const void* bT_all, const float* scale,
-                 const float* row_lse, int b, int n, int d, int k_logits, int target_offset, float eps, void* g_ws,
-                 float* ws_gz, float* grad_a, int n_valid, float coef, cudaStream_t stream);
+int infonce_grad(const void* a_local, const void* b_all, const float* scale, const float* row_lse, int b, int n, int d,
+                 int k_logits, int target_offset, float eps, void* g_ws, float* ws_gz, float* grad_a, int n_valid, float coef,
+                 cudaStream_t stream);
 int infonce_dscale(const float* ws_a, const float* ws_b, int b, int n, float* out, cudaStream_t stream);
 
 // One entry per parameter tensor (device-resident table, 64 bytes; mirrored by ctypes in optim/adam_fused.py)

@@ -350,34 +350,24 @@ def transpose_bf16(x, rows=None, cols=None):
     return out
 
 
-def split_bf16x3(x, side):
-    """fp32 [r,d] -> bf16 [r,3d]; side 0 = [hi|hi|lo] (local operand), side 1 = [hi|lo|hi] (gathered operand)."""
-    _need_cuda(x)
-    assert x.dtype == torch.float32 and x.is_contiguous() and x.dim() == 2
-    r, d = x.shape
-    out = torch.empty(r, 3 * d, dtype=torch.bfloat16, device=x.device)
-    st = _lib.load().opb_split_bf16x3(x.data_ptr(), out.data_ptr(), r, d, side, _stream())
-    _lib.check(st, "opb_split_bf16x3")
-    _count()
-    return out
-
-
-def split_bf16x3_x4(xs, sides):
-    """four fp32 [r_i, d] tensors -> four bf16 [r_i, 3d] splits in ONE launch (the operands of one InfoNCE step)"""
+def split_bf16x3(xs, sides):
+    """fp32 [r_i, d] tensors (1 to 4) -> bf16 [r_i, 3d] splits in ONE launch; side 0 = [hi|hi|lo] (local operand),
+    side 1 = [hi|lo|hi] (gathered operand)."""
     import ctypes
-    assert len(xs) == 4 and len(sides) == 4
+    count = len(xs)
+    assert 1 <= count <= 4 and len(sides) == count
     d = xs[0].shape[1]
     for x in xs:
         _need_cuda(x)
         assert x.dtype == torch.float32 and x.is_contiguous() and x.dim() == 2 and x.shape[1] == d
     outs = [torch.empty(x.shape[0], 3 * d, dtype=torch.bfloat16, device=x.device) for x in xs]
-    px = (ctypes.c_void_p * 4)(*[x.data_ptr() for x in xs])
-    po = (ctypes.c_void_p * 4)(*[o.data_ptr() for o in outs])
-    pr = (ctypes.c_int64 * 4)(*[x.shape[0] for x in xs])
-    ps = (ctypes.c_int * 4)(*[int(v) for v in sides])
-    st = _lib.load().opb_split_bf16x3_x4(ctypes.cast(px, ctypes.c_void_p), ctypes.cast(po, ctypes.c_void_p),
-                                         ctypes.cast(pr, ctypes.c_void_p), ctypes.cast(ps, ctypes.c_void_p), d, _stream())
-    _lib.check(st, "opb_split_bf16x3_x4")
+    px = (ctypes.c_void_p * count)(*[x.data_ptr() for x in xs])
+    po = (ctypes.c_void_p * count)(*[o.data_ptr() for o in outs])
+    pr = (ctypes.c_int64 * count)(*[x.shape[0] for x in xs])
+    ps = (ctypes.c_int * count)(*[int(v) for v in sides])
+    st = _lib.load().opb_split_bf16x3(ctypes.cast(px, ctypes.c_void_p), ctypes.cast(po, ctypes.c_void_p),
+                                      ctypes.cast(pr, ctypes.c_void_p), ctypes.cast(ps, ctypes.c_void_p), count, d, _stream())
+    _lib.check(st, "opb_split_bf16x3")
     _count()
     return outs
 
@@ -385,81 +375,59 @@ def split_bf16x3_x4(xs, sides):
 _TICKETS = {}
 
 
-def infonce_forward2(a3, b3, a_all3, b_all3, scale, target_offset, eps, n_valid=0, rows=False):
-    """Both directions of the InfoNCE forward in 3 launches (two LSE_PARTIAL GEMMs + one merge / reduce kernel).
-    -> (lse_a [b], lse_b [b], out3 = {loss, #correct a->b, #correct b->a}), and with `rows` also the per-row
-    losses [2 b] and arg-max columns int32 [2 b] (direction a, then b)"""
+def infonce_forward(pairs, scale, target_offset, eps, n_valid=0, rows=False):
+    """InfoNCE forward of one direction, pairs = [(a3, b_all3)], or of both, pairs = [(a3, b_all3), (b3, a_all3)]: one
+    LSE_PARTIAL GEMM per direction + one merge / reduce kernel.  a3 bf16 [b,k], b_all3 bf16 [n,k], scale fp32 device scalar.
+    n_valid > 0: only the first n_valid rows of b_all3 are classes (the rest is zero padding to n % 8 == 0).
+    -> ([row_lse [b] per direction], out3 = {mean row loss over all directions, #correct a->b, #correct b->a (0 for one
+    direction)}), and with `rows` also the row losses [dirs * b] and arg-max columns int32 [dirs * b] (direction a, then b)"""
+    dirs = len(pairs)
+    assert dirs in (1, 2)
+    b, k = pairs[0][0].shape
+    n = pairs[0][1].shape[0]
+    _need_cuda(scale)
+    assert scale.dtype == torch.float32
+    for x, y in pairs:
+        _need_cuda(x, y)
+        assert x.dtype == torch.bfloat16 and y.dtype == torch.bfloat16 and x.is_contiguous() and y.is_contiguous()
+        assert x.shape == (b, k) and y.shape == (n, k)
     lib = _lib.load()
-    b, k = a3.shape
-    n = a_all3.shape[0]
-    dev = a3.device
-    ws_a = torch.empty(lib.opb_infonce_ws_floats(b, n), dtype=torch.float32, device=dev)
-    ws_b = torch.empty_like(ws_a)
-    for x, y, ws in ((a3, b_all3, ws_a), (b3, a_all3, ws_b)):
-        st = lib.opb_infonce_lse_gemm(x.data_ptr(), y.data_ptr(), scale.data_ptr(), b, n, k, target_offset, ws.data_ptr(), int(n_valid),
+    dev = pairs[0][0].device
+    ws = []
+    for x, y in pairs:
+        w = torch.empty(lib.opb_infonce_ws_floats(b, n), dtype=torch.float32, device=dev)
+        st = lib.opb_infonce_lse_gemm(x.data_ptr(), y.data_ptr(), scale.data_ptr(), b, n, k, target_offset, w.data_ptr(), int(n_valid),
                                       _stream())
         _lib.check(st, "opb_infonce_lse_gemm")
-    lse_a = torch.empty(b, dtype=torch.float32, device=dev)
-    lse_b = torch.empty(b, dtype=torch.float32, device=dev)
-    loss_ab = torch.empty(2 * b, dtype=torch.float32, device=dev)
-    am_ab = torch.empty(2 * b, dtype=torch.int32, device=dev)
+        ws.append(w)
+    lse = [torch.empty(b, dtype=torch.float32, device=dev) for _ in pairs]
+    loss_ab = torch.empty(dirs * b, dtype=torch.float32, device=dev)
+    am_ab = torch.empty(dirs * b, dtype=torch.int32, device=dev)
     out3 = torch.empty(3, dtype=torch.float32, device=dev)
     key = dev.index if dev.index is not None else torch.cuda.current_device()
     if key not in _TICKETS:
         _TICKETS[key] = torch.zeros(1, dtype=torch.int32, device=dev)       # the kernel leaves it at zero
-    st = lib.opb_infonce_merge_reduce(ws_a.data_ptr(), ws_b.data_ptr(), b, n, int(n_valid), float(eps), target_offset, lse_a.data_ptr(),
-                                      lse_b.data_ptr(), loss_ab.data_ptr(), am_ab.data_ptr(), out3.data_ptr(), _TICKETS[key].data_ptr(),
+    ws_b, lse_b = (ws[1], lse[1]) if dirs == 2 else (None, None)
+    st = lib.opb_infonce_merge_reduce(ws[0].data_ptr(), _ptr(ws_b), b, n, int(n_valid), float(eps), target_offset, lse[0].data_ptr(),
+                                      _ptr(lse_b), loss_ab.data_ptr(), am_ab.data_ptr(), out3.data_ptr(), _TICKETS[key].data_ptr(),
                                       _stream())
     _lib.check(st, "opb_infonce_merge_reduce")
-    _count(3)
+    _count(dirs + 1)
     if rows:
-        return lse_a, lse_b, out3, loss_ab, am_ab
-    return lse_a, lse_b, out3
+        return lse, out3, loss_ab, am_ab
+    return lse, out3
 
 
-def infonce_rows(a_local, b_all, scale, target_offset, eps, n_valid=0):
-    """One direction of the InfoNCE forward.  a_local bf16 [b,k], b_all bf16 [n,k], scale fp32 device scalar.
-    n_valid > 0: only the first n_valid rows of b_all are classes (the rest is zero padding to n % 8 == 0).
-    -> (row_lse [b], row_loss [b], row_argmax int32 [b])"""
-    _need_cuda(a_local, b_all, scale)
-    b, d = a_local.shape
-    n = b_all.shape[0]
-    assert a_local.dtype == torch.bfloat16 and b_all.dtype == torch.bfloat16 and scale.dtype == torch.float32
-    assert a_local.is_contiguous() and b_all.is_contiguous() and b_all.shape[1] == d
-    lib = _lib.load()
-    dev = a_local.device
-    ws = torch.empty(lib.opb_infonce_ws_floats(b, n), dtype=torch.float32, device=dev)
-    lse = torch.empty(b, dtype=torch.float32, device=dev)
-    loss = torch.empty(b, dtype=torch.float32, device=dev)
-    amax = torch.empty(b, dtype=torch.int32, device=dev)
-    st = lib.opb_infonce_rows(a_local.data_ptr(), b_all.data_ptr(), scale.data_ptr(), b, n, d, target_offset, eps,
-                              ws.data_ptr(), lse.data_ptr(), loss.data_ptr(), amax.data_ptr(), int(n_valid), _stream())
-    _lib.check(st, "opb_infonce_rows")
-    _count(2)
-    return lse, loss, amax
-
-
-def infonce_reduce(loss_a, loss_b, am_a, am_b, target_offset):
-    out = torch.empty(3, dtype=torch.float32, device=loss_a.device)
-    st = _lib.load().opb_infonce_reduce(loss_a.data_ptr(), loss_b.data_ptr(), am_a.data_ptr(), am_b.data_ptr(),
-                                        loss_a.numel(), target_offset, out.data_ptr(), _stream())
-    _lib.check(st, "opb_infonce_reduce")
-    _count()
-    return out
-
-
-def infonce_grad(a_local, b_all, bT_all, scale, row_lse, target_offset, eps, n_valid=0, coef=0.0, d=None):
-    """-> (grad_a fp32 [b,d], ws_gz) for one direction; a_local/b_all [.,k] (k = d or 3d).  bT_all: bf16 [d,n] transposed copy
-    of b_all's first d columns, or None (then pass d): b_all is read in place as an MN-major operand.
-    coef = weight of one row's loss (0 -> 1 / (2 b), the two-direction InfoNCE mean)"""
+def infonce_grad(a_local, b_all, scale, row_lse, target_offset, eps, d, n_valid=0, coef=0.0):
+    """-> (grad_a fp32 [b,d], ws_gz) for one direction; a_local/b_all [.,k] (k = d or 3d); b_all is read in place as an
+    MN-major operand.  coef = weight of one row's loss (0 -> 1 / (2 b), the two-direction InfoNCE mean)"""
     b, k = a_local.shape
     n = b_all.shape[0]
-    d = bT_all.shape[0] if bT_all is not None else int(d)
     dev = a_local.device
     g_ws = torch.empty(b, n, dtype=torch.bfloat16, device=dev)
     ws_gz = torch.empty((n + 255) // 256 * b, dtype=torch.float32, device=dev)
     grad = torch.empty(b, d, dtype=torch.float32, device=dev)
-    st = _lib.load().opb_infonce_grad(a_local.data_ptr(), b_all.data_ptr(), _ptr(bT_all), scale.data_ptr(),
+    st = _lib.load().opb_infonce_grad(a_local.data_ptr(), b_all.data_ptr(), scale.data_ptr(),
                                       row_lse.data_ptr(), b, n, d, k, target_offset, eps, g_ws.data_ptr(),
                                       ws_gz.data_ptr(), grad.data_ptr(), int(n_valid), float(coef), _stream())
     _lib.check(st, "opb_infonce_grad")

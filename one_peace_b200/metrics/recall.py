@@ -58,8 +58,7 @@ class Recall:
     @staticmethod
     def _similarity(a, b):
         """fp32 [Na, Nb] = a b^T through the wgmma GEMM on bf16x3-split operands."""
-        a3 = K.split_bf16x3(a.detach().float().contiguous(), 0)
-        b3 = K.split_bf16x3(b.detach().float().contiguous(), 1)
+        a3, b3 = K.split_bf16x3([a.detach().float().contiguous(), b.detach().float().contiguous()], [0, 1])
         nb = b.shape[0]
         nb8 = (nb + 7) // 8 * 8                       # the GEMM wants N % 8 == 0: zero rows, never ranked (C = nb below)
         if nb8 != nb:

@@ -1,7 +1,7 @@
 """GPU: the contrastive-head kernels (csrc/infonce.cu and the LSE_PARTIAL / SOFTMAX_GRAD GEMM epilogues) row by row against
 the fp64 reference of tests/kernel_ref.py, which starts from the fp32 features: the bf16x3 split, the per-tile partials
 and their merge across several column tiles (targets in later tiles, a padded last tile, arg-max ties across tiles), the
-ticket-based reduction of infonce_forward2, the gradient G . B_hi, d loss / d logit_scale and the plain reduction."""
+ticket-based reduction of infonce_forward over one and two directions, the gradient G . B_hi and d loss / d logit_scale."""
 import pytest
 import torch
 
@@ -20,7 +20,7 @@ def K():
     return kernels
 
 
-def features(b, n, n_valid, offset, seed):
+def features(b, n, n_valid, offset, seed, noise=0.8):
     """local rows a, b [b, D] and gathered rows a_all, b_all [n, D] (local rows at `offset`, zero rows from n_valid on)"""
     g = torch.Generator(device="cuda").manual_seed(seed)
     nrm = torch.nn.functional.normalize
@@ -28,25 +28,36 @@ def features(b, n, n_valid, offset, seed):
     a_all = torch.zeros(n, D, device="cuda")
     b_all = torch.zeros(n, D, device="cuda")
     a_all[:n_cls] = nrm(torch.randn(n_cls, D, device="cuda", generator=g), dim=1)
-    b_all[:n_cls] = nrm(a_all[:n_cls] + 0.8 * torch.randn(n_cls, D, device="cuda", generator=g), dim=1)
+    b_all[:n_cls] = nrm(a_all[:n_cls] + noise * torch.randn(n_cls, D, device="cuda", generator=g), dim=1)
     return a_all[offset:offset + b].clone(), b_all[offset:offset + b].clone(), a_all, b_all
 
 
 def splits(K, xa, xb, xa_all, xb_all):
-    return K.split_bf16x3_x4([xa, xb, xa_all, xb_all], [0, 0, 1, 1])
+    return K.split_bf16x3([xa, xb, xa_all, xb_all], [0, 0, 1, 1])
 
 
-def test_split_bf16x3_x4_layouts(K):
+def both(a3, b3, a_all3, b_all3):
+    return [(a3, b_all3), (b3, a_all3)]
+
+
+def flat(res):
+    """infonce_forward's result as a flat tuple of tensors"""
+    return (*res[0], *res[1:])
+
+
+def test_split_bf16x3_layouts(K):
+    """1, 2 and 4 tensors per launch"""
     g = torch.Generator(device="cuda").manual_seed(3)
     xs = [torch.randn(r, D, device="cuda", generator=g) * 10.0 ** torch.empty(r, 1, device="cuda").uniform_(-20, 20, generator=g)
           for r in (37, 200, 800, 3)]
     sides = [0, 1, 1, 0]
-    outs = K.split_bf16x3_x4(xs, sides)
-    for x, side, o in zip(xs, sides, outs):
-        hi = x.bfloat16()
-        lo = (x - hi.float()).bfloat16()
-        want = torch.cat([hi, hi, lo] if side == 0 else [hi, lo, hi], 1)
-        assert torch.equal(o.view(torch.int16), want.view(torch.int16))
+    for count in (1, 2, 4):
+        outs = K.split_bf16x3(xs[:count], sides[:count])
+        for x, side, o in zip(xs, sides, outs):
+            hi = x.bfloat16()
+            lo = (x - hi.float()).bfloat16()
+            want = torch.cat([hi, hi, lo] if side == 0 else [hi, lo, hi], 1)
+            assert torch.equal(o.view(torch.int16), want.view(torch.int16)), f"{count} tensor(s)"
 
 
 def check_direction(K, ref, lse, loss, am, what):
@@ -60,7 +71,7 @@ def check_direction(K, ref, lse, loss, am, what):
 @pytest.mark.parametrize("eps", [0.0, 0.1])
 @pytest.mark.parametrize("n,n_valid", [(800, 0), (800, 789)])
 @pytest.mark.parametrize("b", [37, 200, 300])
-def test_forward_and_gradient(K, b, n, n_valid, eps):
+def test_forward_one_and_two_directions_and_gradient(K, b, n, n_valid, eps):
     """n = 800: four 256-column tiles, the last one partly padding; targets start at column 300 (tile 1 and later)"""
     off = 300
     xa, xb, xa_all, xb_all = features(b, n, n_valid, off, seed=b + n_valid)
@@ -69,7 +80,8 @@ def test_forward_and_gradient(K, b, n, n_valid, eps):
     ref_a = R.infonce_ref(xa, xb_all, SCALE, off, eps, n_valid)
     ref_b = R.infonce_ref(xb, xa_all, SCALE, off, eps, n_valid)
 
-    lse_a, lse_b, out3, loss_ab, am_ab = K.infonce_forward2(a3, b3, a_all3, b_all3, scale, off, eps, n_valid=n_valid, rows=True)
+    first = K.infonce_forward(both(a3, b3, a_all3, b_all3), scale, off, eps, n_valid=n_valid, rows=True)
+    (lse_a, lse_b), out3, loss_ab, am_ab = first
     check_direction(K, ref_a, lse_a, loss_ab[:b], am_ab[:b], "a->b")
     check_direction(K, ref_b, lse_b, loss_ab[b:], am_ab[b:], "b->a")
     tgt = torch.arange(b, device="cuda") + off
@@ -77,18 +89,23 @@ def test_forward_and_gradient(K, b, n, n_valid, eps):
     mean = (ref_a.loss.sum() + ref_b.loss.sum()) / (2 * b)
     tol = (ref_a.dloss.sum() + ref_b.dloss.sum() + 2.0 ** -16 * (ref_a.loss.abs().sum() + ref_b.loss.abs().sum())) / (2 * b)
     R.assert_within(out3[:1], mean.view(1), tol.view(1), 1.0, torch.float32, what="mean loss")
-    again = K.infonce_forward2(a3, b3, a_all3, b_all3, scale, off, eps, n_valid=n_valid, rows=True)
-    for x, y in zip((lse_a, lse_b, out3, loss_ab, am_ab), again):
+    again = K.infonce_forward(both(a3, b3, a_all3, b_all3), scale, off, eps, n_valid=n_valid, rows=True)
+    for x, y in zip(flat(first), flat(again)):
         assert torch.equal(x, y)
 
-    # the one-direction merge kernel
-    lse1, loss1, am1 = K.infonce_rows(a3, b_all3, scale, off, eps, n_valid=n_valid)
-    check_direction(K, ref_a, lse1, loss1, am1, "infonce_rows")
+    # one direction: the rows of direction a, bit for bit, and their own mean and hit count
+    (lse1,), out1, loss1, am1 = K.infonce_forward([(a3, b_all3)], scale, off, eps, n_valid=n_valid, rows=True)
+    check_direction(K, ref_a, lse1, loss1, am1, "one direction")
+    assert torch.equal(lse1, lse_a) and torch.equal(loss1, loss_ab[:b]) and torch.equal(am1, am_ab[:b])
+    assert out1[1].item() == (am1 == tgt).sum().item() and out1[2].item() == 0
+    mean1 = ref_a.loss.sum() / b
+    tol1 = (ref_a.dloss.sum() + 2.0 ** -16 * ref_a.loss.abs().sum()) / b
+    R.assert_within(out1[:1], mean1.view(1), tol1.view(1), 1.0, torch.float32, what="one-direction mean loss")
 
     # gradient through the MN-major G . B_all contraction, and d loss / d logit_scale
     coef = 1.0 / (2 * b)
-    grad_a, gz_a = K.infonce_grad(a3, b_all3, None, scale, lse_a, off, eps, n_valid=n_valid, d=D)
-    grad_b, gz_b = K.infonce_grad(b3, a_all3, None, scale, lse_b, off, eps, n_valid=n_valid, d=D)
+    grad_a, gz_a = K.infonce_grad(a3, b_all3, scale, lse_a, off, eps, D, n_valid=n_valid)
+    grad_b, gz_b = K.infonce_grad(b3, a_all3, scale, lse_b, off, eps, D, n_valid=n_valid)
     for ref, grad, xo, what in ((ref_a, grad_a, xb_all, "grad a"), (ref_b, grad_b, xa_all, "grad b")):
         want, tol = R.infonce_grad_ref(ref, xo.bfloat16(), SCALE, coef)
         R.assert_within(grad, want, tol, 1.0, torch.float32, what=what)
@@ -101,7 +118,7 @@ def test_forward_and_gradient(K, b, n, n_valid, eps):
     R.assert_within(ds, want.view(1), tol.view(1), 1.0, torch.float32, what="dscale")
 
 
-def test_argmax_tie_across_tiles(K):
+def test_argmax_tie_across_tiles_one_and_two_directions(K):
     """the same gathered row at columns 100 (tile 0) and 300 (tile 1), the best match of local row 5: the lower index wins,
     as torch.argmax picks it"""
     b, n = 37, 512
@@ -110,43 +127,44 @@ def test_argmax_tie_across_tiles(K):
     xb_all[300] = xa[5]
     a3, b3, a_all3, b_all3 = splits(K, xa, xb, xa_all, xb_all)
     scale = torch.tensor([SCALE], device="cuda")
-    _, _, _, _, am_ab = K.infonce_forward2(a3, b3, a_all3, b_all3, scale, 0, 0.0, rows=True)
+    *_, am_ab = K.infonce_forward(both(a3, b3, a_all3, b_all3), scale, 0, 0.0, rows=True)
     assert am_ab[5].item() == 100
-    _, _, am1 = K.infonce_rows(a3, b_all3, scale, 0, 0.0)
+    *_, am1 = K.infonce_forward([(a3, b_all3)], scale, 0, 0.0, rows=True)
     assert am1[5].item() == 100
     z = SCALE * (xa.double() @ xb_all.double().t())
     assert z[5].argmax().item() == 100
 
 
-def test_forward2_ticket_is_reset(K):
-    """three calls in a row with different b (so different grids) give what fresh calls give: the last block of each call
-    returns the ticket counter to zero"""
+def test_forward_ticket_is_reset(K):
+    """calls in a row with different b and direction counts (so different grids) give what fresh calls give: the last block
+    of each call returns the ticket counter to zero"""
     n, off = 512, 100
     scale = torch.tensor([SCALE], device="cuda")
+    calls = [(37, 2), (300, 1), (200, 2), (37, 1), (300, 2)]
     args = {}
     for b in (37, 300, 200):
         xs = features(b, n, 0, off, seed=b)
-        args[b] = splits(K, *xs)
-    seq = {b: K.infonce_forward2(*args[b], scale, off, 0.1, rows=True) for b in (37, 300, 200)}
-    for b in (37, 300, 200):
+        args[b] = both(*splits(K, *xs))
+    seq = [K.infonce_forward(args[b][:dirs], scale, off, 0.1, rows=True) for b, dirs in calls]
+    for (b, dirs), got in zip(calls, seq):
         K._TICKETS.clear()                                  # a fresh zero ticket
-        fresh = K.infonce_forward2(*args[b], scale, off, 0.1, rows=True)
-        for x, y in zip(seq[b], fresh):
-            assert torch.equal(x, y), f"b = {b}"
+        fresh = K.infonce_forward(args[b][:dirs], scale, off, 0.1, rows=True)
+        for x, y in zip(flat(got), flat(fresh)):
+            assert torch.equal(x, y), f"b = {b}, {dirs} direction(s)"
 
 
-def test_infonce_reduce_many_rows(K):
-    """b > 1024: more rows than the single block has threads"""
-    b, off = 3000, 500
-    g = torch.Generator(device="cuda").manual_seed(11)
-    la = torch.rand(b, device="cuda", generator=g) * 8
-    lb = torch.rand(b, device="cuda", generator=g) * 8
+def test_forward_many_rows(K):
+    """b = 3000, one and two directions: many more rows than the reducing block has threads; out3 is the mean of the call's
+    own row losses and its hit counts are those of its own arg-max rows"""
+    b, n, off = 3000, 3504, 500
+    xs = features(b, n, 0, off, seed=11, noise=0.25)
+    scale = torch.tensor([SCALE], device="cuda")
     tgt = torch.arange(b, device="cuda", dtype=torch.int32) + off
-    hit_a = torch.rand(b, device="cuda", generator=g) < 0.3
-    hit_b = torch.rand(b, device="cuda", generator=g) < 0.6
-    am_a = torch.where(hit_a, tgt, tgt + 1).int().contiguous()
-    am_b = torch.where(hit_b, tgt, tgt - 1).int().contiguous()
-    out = K.infonce_reduce(la, lb, am_a, am_b, off)
-    want = (la.double().sum() + lb.double().sum()) / (2 * b)
-    R.assert_within(out[:1], want.view(1), want.view(1), R.TAU, torch.float32, what="mean loss")
-    assert out[1].item() == hit_a.sum().item() and out[2].item() == hit_b.sum().item()
+    for dirs in (1, 2):
+        pairs = both(*splits(K, *xs))[:dirs]
+        _, out, loss_ab, am_ab = K.infonce_forward(pairs, scale, off, 0.1, rows=True)
+        want = loss_ab.double().sum() / (dirs * b)
+        R.assert_within(out[:1], want.view(1), want.view(1), R.TAU, torch.float32, what=f"mean loss, {dirs} direction(s)")
+        hits = [(am_ab[i * b:(i + 1) * b] == tgt).sum().item() for i in range(dirs)] + [0] * (2 - dirs)
+        assert 0 < hits[0] < b, "the inputs should give some hits and some misses"
+        assert out[1].item() == hits[0] and out[2].item() == hits[1], f"{dirs} direction(s)"

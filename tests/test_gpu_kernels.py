@@ -568,7 +568,7 @@ def test_attention_tc_two_segments(K):
     assert relerr(out, want) < 2e-2
 
 
-def test_dcl_form_of_infonce_kernels(K):
+def test_dcl_form_of_one_direction_infonce_forward(K):
     """n_valid / coef form: single-direction label-smoothed NLL over a ragged number of classes
     (compute_dcl_loss, image_text_pretrain_loss.py:187-208)."""
     g = torch.Generator(device="cuda").manual_seed(15)
@@ -580,8 +580,8 @@ def test_dcl_form_of_infonce_kernels(K):
     tea_p = torch.zeros(n8, d, device="cuda")
     tea_p[:nt] = tea
     scale = torch.tensor([2.5], device="cuda")
-    a3, b3 = K.split_bf16x3(stu, 0), K.split_bf16x3(tea_p, 1)
-    lse, loss, am = K.infonce_rows(a3, b3, scale, 0, 0.1, n_valid=nt)
+    a3, b3 = K.split_bf16x3([stu, tea_p], [0, 1])
+    (lse,), out3, loss, am = K.infonce_forward([(a3, b3)], scale, 0, 0.1, n_valid=nt, rows=True)
     sa = stu.clone().requires_grad_(True)
     sim = 2.5 * sa @ tea.t()
     lp = torch.log_softmax(sim, -1)
@@ -590,8 +590,9 @@ def test_dcl_form_of_infonce_kernels(K):
     eps_i = 0.1 / (nt - 1)
     want_rows = (1 - 0.1 - eps_i) * nll + eps_i * (-lp.sum(-1))
     torch.testing.assert_close(loss, want_rows.detach(), atol=2e-4, rtol=2e-4)
+    torch.testing.assert_close(out3[0], want_rows.detach().mean(), atol=2e-4, rtol=2e-4)
     assert torch.equal(am.long(), sim.argmax(1))
-    grad, _ = K.infonce_grad(a3, b3, K.transpose_bf16(b3, cols=d), scale, lse, 0, 0.1, n_valid=nt, coef=1.0 / nm)
+    grad, _ = K.infonce_grad(a3, b3, scale, lse, 0, 0.1, d, n_valid=nt, coef=1.0 / nm)
     want_rows.mean().backward()
     assert relerr(grad, sa.grad) < 2e-2
 
