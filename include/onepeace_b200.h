@@ -565,6 +565,30 @@ int64_t opb_average_precision_ws_bytes(int N, int C);
 int opb_average_precision(const float* probs, const uint8_t* labels, int N, int C, void* ws, int64_t ws_bytes, double* ap,
                           double* mean, int64_t* npos, void* stream);
 
+/* ------------------------------------------------------------------------------------------------------------------
+ * Pooled head of OnePeaceViT (one_peace_vision/classification/models_vit.py:431-434, global_pool=True).
+ *   opb_token_mean_ln_ws_floats : floats of the forward's workspace for (B, S, d); -1 for a shape the kernels refuse.
+ *   opb_token_mean_ln_fwd : m[b] = mean of x[b, 1:S, :] over the S - 1 patch rows (the CLS row 0 is excluded; the sum is
+ *                           divided by S - 1), then fc_norm: y[b] = bf16((m[b] - mean[b]) * rstd[b] * gamma + beta) with
+ *                           mean[b] / rstd[b] = the LayerNorm statistics of m[b] over d (biased variance, rstd =
+ *                           1 / sqrt(var + eps)).  x fp32, row (b, s) at x + (b * S + s) * ld; m fp32 [B, d] (kept for the
+ *                           backward), y bf16 [B, d] (the A operand of the head GEMM), mean / rstd fp32 [B].  The row sum is
+ *                           split across CTAs per (sample, 256-column slice, row range) into ws and merged in split order by
+ *                           one CTA per sample: the split count depends on the shape only, there are no atomics, and repeated
+ *                           launches are bit-identical.
+ *   opb_token_mean_ln_bwd : its adjoint for dy = d loss / d y fp32 [B, d]: dgamma / dbeta fp32 [d] summed over b in order;
+ *                           dx fp32 (row (b, s) at dx + (b * S + s) * ld_dx) = the LayerNorm adjoint of row b divided by
+ *                           S - 1 in every patch row s >= 1 and exact zeros in the CLS row s = 0.  Every row of dx is
+ *                           written exactly once, so it needs no zeroing.  ws: fp32 [B, d] scratch.
+ * Both need 1 <= B <= 65535, S >= 2, d >= 4 with d % 4 == 0, a row pitch >= d with pitch % 4 == 0, x / dx / ws 16-byte
+ * aligned, eps >= 0 and a large enough workspace; anything else (or a null pointer) returns status 1 before any launch.
+ * ------------------------------------------------------------------------------------------------------------------ */
+int64_t opb_token_mean_ln_ws_floats(int B, int S, int d);
+int opb_token_mean_ln_fwd(const float* x, int64_t ld, int B, int S, int d, const float* gamma, const float* beta, float eps,
+                          float* ws, int64_t ws_floats, float* m, void* y, float* mean, float* rstd, void* stream);
+int opb_token_mean_ln_bwd(const float* dy, const float* m, const float* mean, const float* rstd, const float* gamma, int B,
+                          int S, int d, float* dgamma, float* dbeta, float* ws, float* dx, int64_t ld_dx, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -111,6 +111,11 @@ SIGNATURES.update({
     "opb_average_precision_ws_bytes": (c_int64, [c_int, c_int]),
     "opb_average_precision": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_int64, c_void_p, c_void_p, c_void_p,
                                       c_void_p]),
+    "opb_token_mean_ln_ws_floats": (c_int64, [c_int, c_int, c_int]),
+    "opb_token_mean_ln_fwd": (c_int, [c_void_p, c_int64, c_int, c_int, c_int, c_void_p, c_void_p, c_float, c_void_p, c_int64,
+                                      c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "opb_token_mean_ln_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p,
+                                      c_void_p, c_void_p, c_int64, c_void_p]),
 })
 
 

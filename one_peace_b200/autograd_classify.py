@@ -194,3 +194,60 @@ class RefcocoLossFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, g_loss, _g1, _g2):
         return (ctx.dl * g_loss.to(torch.float32)).to(ctx.dtype), None, None
+
+
+class VitHeadFn(torch.autograd.Function):
+    """Head of OnePeaceViT (one_peace_vision/classification/models_vit.py:431-434): the last layer's residual stream x fp32
+    [B, S, d] -> logits fp32 [B, num_classes].
+
+      global_pool : mean over the S - 1 patch rows -> fc_norm       (opb_token_mean_ln_fwd / _bwd, csrc/vit_head.cu)
+      otherwise   : encoder.layer_norm on the CLS row                (opb_layernorm / opb_layernorm_bwd at a row pitch of S * d)
+      then head (GEMM, output rows zero-padded to a multiple of 8).
+
+    meta = (pack, global_pool, norm eps); then norm weight, norm bias, head weight, head bias.  The gradient of x is written
+    whole by the kernels: the pooled form's backward writes every row, the CLS form's its rows into a zeroed buffer."""
+
+    @staticmethod
+    def forward(ctx, meta, x, nw, nb, w, b):
+        pk, pool, eps = meta
+        B, S, d = x.shape
+        dev = x.device
+        x = x.contiguous()
+        if pool:
+            a, m, mean, rstd = K.token_mean_ln_fwd(x, pk["norm_w"], pk["norm_b"], eps)
+            ctx.saved = (m, mean, rstd)
+        else:
+            a = K.layernorm(x, pk["norm_w"], pk["norm_b"], torch.empty(B, d, dtype=torch.bfloat16, device=dev), rows=B, dim=d,
+                            ld_in=S * d, ld_out=d, eps=eps)
+            ctx.saved = (x,)
+        logits = K.gemm(a, pk["w"], K.EPI_STORE_F32, torch.empty(B, pk["w"].shape[0], dtype=torch.float32, device=dev),
+                        bias=pk["b"])
+        ctx.meta = (pk, pool, eps, B, S, d)
+        ctx.a = a
+        ctx.dtypes = (nw.dtype, nb.dtype, w.dtype, b.dtype)
+        return logits[:, :pk["n_cls"]]
+
+    @staticmethod
+    def backward(ctx, dlogits):
+        pk, pool, eps, B, S, d = ctx.meta
+        dev = dlogits.device
+        n_cls, n_pad = pk["n_cls"], pk["w"].shape[0]
+        dl = torch.zeros(B, n_pad, dtype=torch.bfloat16, device=dev)
+        dl[:, :n_cls].copy_(dlogits)
+        db = K.colsum(dl, torch.empty(n_pad, dtype=torch.float32, device=dev))[:n_cls]
+        dW = _dw(dl, ctx.a, torch.float32)[:n_cls]
+        da = _dx(dl, pk["w"], d, out=torch.empty(B, d, dtype=torch.float32, device=dev))
+        if pool:
+            m, mean, rstd = ctx.saved
+            dx = torch.empty(B, S, d, dtype=torch.float32, device=dev)
+            dnw, dnb = K.token_mean_ln_bwd(da, m, mean, rstd, pk["norm_w"], dx)
+        else:
+            (x,) = ctx.saved
+            dx = torch.zeros(B, S, d, dtype=torch.float32, device=dev)
+            dnw = torch.empty(d, dtype=torch.float32, device=dev)
+            dnb = torch.empty(d, dtype=torch.float32, device=dev)
+            K.layernorm_bwd(x, da, pk["norm_w"], pk["norm_b"], dx, eps=eps, dgamma=dnw, dbeta=dnb, rows=B, dim=d, ldx=S * d,
+                            ld_dx=S * d)
+        ctx.saved = ctx.a = None
+        grads = [g.to(dt) for g, dt in zip((dnw, dnb, dW, db), ctx.dtypes)]
+        return (None, dx, *grads)

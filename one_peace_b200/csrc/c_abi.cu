@@ -465,4 +465,20 @@ int opb_average_precision(const float* probs, const uint8_t* labels, int N, int 
   return opb::average_precision(probs, labels, N, C, ws, ws_bytes, ap, mean, npos, static_cast<cudaStream_t>(stream));
 }
 
+int64_t opb_token_mean_ln_ws_floats(int B, int S, int d) { return opb::token_mean_ln_ws_floats(B, S, d); }
+
+int opb_token_mean_ln_fwd(const float* x, int64_t ld, int B, int S, int d, const float* gamma, const float* beta, float eps,
+                          float* ws, int64_t ws_floats, float* m, void* y, float* mean, float* rstd, void* stream) {
+  if (!x || !gamma || !beta || !ws || !m || !y || !mean || !rstd) return OPB_ERR_INVALID;
+  return opb::token_mean_ln_fwd(x, ld, B, S, d, gamma, beta, eps, ws, ws_floats, m, y, mean, rstd,
+                                static_cast<cudaStream_t>(stream));
+}
+
+int opb_token_mean_ln_bwd(const float* dy, const float* m, const float* mean, const float* rstd, const float* gamma, int B,
+                          int S, int d, float* dgamma, float* dbeta, float* ws, float* dx, int64_t ld_dx, void* stream) {
+  if (!dy || !m || !mean || !rstd || !gamma || !dgamma || !dbeta || !ws || !dx) return OPB_ERR_INVALID;
+  return opb::token_mean_ln_bwd(dy, m, mean, rstd, gamma, B, S, d, dgamma, dbeta, ws, dx, ld_dx,
+                                static_cast<cudaStream_t>(stream));
+}
+
 }  // extern "C"

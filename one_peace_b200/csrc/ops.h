@@ -197,4 +197,11 @@ long average_precision_ws_bytes(int N, int C);
 int average_precision(const float* probs, const uint8_t* labels, int N, int C, void* ws, long ws_bytes, double* ap,
                       double* mean, int64_t* npos, cudaStream_t stream);
 
+// csrc/vit_head.cu: the pooled head of OnePeaceViT (mean over the patch rows + fc_norm) and its adjoint
+long token_mean_ln_ws_floats(int B, int S, int d);
+int token_mean_ln_fwd(const float* x, long ld, int B, int S, int d, const float* gamma, const float* beta, float eps, float* ws,
+                      long ws_floats, float* m, void* y, float* mean, float* rstd, cudaStream_t stream);
+int token_mean_ln_bwd(const float* dy, const float* m, const float* mean, const float* rstd, const float* gamma, int B, int S,
+                      int d, float* dgamma, float* dbeta, float* ws, float* dx, long ld_dx, cudaStream_t stream);
+
 }  // namespace opb

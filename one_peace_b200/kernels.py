@@ -957,3 +957,57 @@ def average_precision(probs, labels):
     _lib.check(st, "opb_average_precision")
     _count(4 + 3 * ((31 + max(C - 1, 0).bit_length() + 7) // 8))
     return ap, mean, npos
+
+
+# ----------------------------------------------------------------------------------------------------------------
+# pooled head of OnePeaceViT (csrc/vit_head.cu)
+# ----------------------------------------------------------------------------------------------------------------
+def _check_rows3(x, name):
+    """(B, S, d, row pitch) of an fp32 [B, S, d] view whose rows are d contiguous floats at one pitch."""
+    if x.dtype != torch.float32 or x.dim() != 3 or x.stride(2) != 1 or x.stride(0) != x.shape[1] * x.stride(1):
+        raise ValueError(f"{name}: fp32 [B, S, d] with unit column stride and one row pitch expected")
+    return x.shape[0], x.shape[1], x.shape[2], x.stride(1)
+
+
+def token_mean_ln_fwd(x, gamma, beta, eps):
+    """x fp32 [B, S, d] (any row pitch) -> (y bf16 [B, d], m fp32 [B, d], mean fp32 [B], rstd fp32 [B]):
+    y = LayerNorm(x[:, 1:].mean(1)) with gamma / beta fp32 [d] (models_vit.py:431-434, global_pool=True)."""
+    _need_cuda(x, gamma, beta)
+    B, S, d, ld = _check_rows3(x, "token_mean_ln_fwd")
+    for t in (gamma, beta):
+        if t.dtype != torch.float32 or not t.is_contiguous() or t.numel() != d:
+            raise ValueError("token_mean_ln_fwd: gamma / beta must be contiguous fp32 [d]")
+    lib = _lib.load()
+    n_ws = lib.opb_token_mean_ln_ws_floats(B, S, d)
+    if n_ws < 0:
+        raise ValueError(f"token_mean_ln_fwd: unsupported shape B={B}, S={S}, d={d}")
+    dev = x.device
+    ws = torch.empty(n_ws, dtype=torch.float32, device=dev)
+    m = torch.empty(B, d, dtype=torch.float32, device=dev)
+    y = torch.empty(B, d, dtype=torch.bfloat16, device=dev)
+    mean = torch.empty(B, dtype=torch.float32, device=dev)
+    rstd = torch.empty(B, dtype=torch.float32, device=dev)
+    st = lib.opb_token_mean_ln_fwd(x.data_ptr(), ld, B, S, d, gamma.data_ptr(), beta.data_ptr(), float(eps), ws.data_ptr(), n_ws,
+                                   m.data_ptr(), y.data_ptr(), mean.data_ptr(), rstd.data_ptr(), _stream())
+    _lib.check(st, "opb_token_mean_ln_fwd")
+    _count(2)
+    return y, m, mean, rstd
+
+
+def token_mean_ln_bwd(dy, m, mean, rstd, gamma, dx):
+    """Adjoint of token_mean_ln_fwd for dy fp32 [B, d]: writes dx fp32 [B, S, d] (any row pitch; every row, the CLS row as
+    zeros) and returns (dgamma fp32 [d], dbeta fp32 [d])."""
+    _need_cuda(dy, m, mean, rstd, gamma, dx)
+    B, S, d, ld = _check_rows3(dx, "token_mean_ln_bwd")
+    for t, shape in ((dy, (B, d)), (m, (B, d)), (mean, (B,)), (rstd, (B,)), (gamma, (d,))):
+        if t.dtype != torch.float32 or not t.is_contiguous() or tuple(t.shape) != shape:
+            raise ValueError(f"token_mean_ln_bwd: contiguous fp32 operands of shape {shape} expected, got {tuple(t.shape)}")
+    dev = dy.device
+    dgamma = torch.empty(d, dtype=torch.float32, device=dev)
+    dbeta = torch.empty(d, dtype=torch.float32, device=dev)
+    ws = torch.empty(B, d, dtype=torch.float32, device=dev)
+    st = _lib.load().opb_token_mean_ln_bwd(dy.data_ptr(), m.data_ptr(), mean.data_ptr(), rstd.data_ptr(), gamma.data_ptr(), B, S, d,
+                                           dgamma.data_ptr(), dbeta.data_ptr(), ws.data_ptr(), dx.data_ptr(), ld, _stream())
+    _lib.check(st, "opb_token_mean_ln_bwd")
+    _count(2)
+    return dgamma, dbeta
