@@ -71,6 +71,9 @@ class Recall:
     def retrieval_eval(self, output_predict=False):
         img_ids, txt_ids = self.image_ids.to(torch.int64).contiguous(), self.text_ids.to(torch.int64).contiguous()
         n_img, n_txt = self.image_logits.shape[0], self.text_logits.shape[0]
+        if min(n_img, n_txt) < 10:                     # the reference's topk(k=10) raises here too (recall.py:39,50)
+            raise RuntimeError(f"Recall@10 needs at least 10 candidates in each direction; got {n_txt} texts and "
+                               f"{n_img} images")
         rank_txt = K.topk10_rows(self._similarity(self.image_logits, self.text_logits))      # image -> text
         rank_img = K.topk10_rows(self._similarity(self.text_logits, self.image_logits))      # text -> image
         i2t = K.recall_hits(rank_txt, txt_ids, img_ids).tolist()
@@ -80,8 +83,8 @@ class Recall:
         tr_mean, ir_mean = sum(tr) / 3, sum(ir) / 3
         predict_txt, predict_img = {}, {}
         if output_predict:
-            pt = txt_ids[rank_txt.clamp_min(0).long()].cpu().tolist()
-            pi = img_ids[rank_img.clamp_min(0).long()].cpu().tolist()
+            pt = txt_ids[rank_txt.long()].cpu().tolist()
+            pi = img_ids[rank_img.long()].cpu().tolist()
             predict_txt = dict(zip(img_ids.cpu().tolist(), pt))
             predict_img = dict(zip(txt_ids.cpu().tolist(), pi))
         return {"txt_r1": tr[0], "txt_r5": tr[1], "txt_r10": tr[2], "txt_r_mean": tr_mean, "img_count": n_img,

@@ -1,8 +1,9 @@
 """fp64 references of the GEMM epilogues (csrc/gemm_wgmma.cu) and of the convolutions lowered onto that GEMM, of the
 contrastive-head reductions (csrc/infonce.cu), of the attention forward and backward (csrc/attention.cu,
 csrc/attention_bwd.cu) and of the row kernels (csrc/layernorm.cu, csrc/backward.cu, csrc/pack.cu, csrc/gather.cu), with an
-error bound for every output element, and NaN-canary output buffers; and of the fused Adam step and the gradient norm
-(csrc/adam.cu).
+error bound for every output element, and NaN-canary output buffers; of the fused Adam step and the gradient norm
+(csrc/adam.cu); and of the embedding, gather, transpose and ranking kernels (csrc/adapters.cu, csrc/gather.cu,
+csrc/infonce.cu, csrc/recall.cu), most of them exact.
 
 Plain PyTorch on whatever device the inputs live on; nothing here calls the extension.
 
@@ -52,9 +53,11 @@ absolute (``assert_within(got, ref, bound, 1.0, dtype)``; a bf16 output adds u_o
            few ulps of |s| and |lse| and stays under 32 ulps of (1 + |s| + |lse|).  eps_b = 0 for the fp32 bias forms.
            The transposed half2 tables of the backward hold fp16(b log2 e): eps_b = 2^-11 + 2^-22 (round-to-nearest to 11
            bits, then the fp32 products), plus an absolute 2^-24 for fp16 subnormals (``EPS_B_HALF``).
-``lse``    sum_j P_ij e_ij + 2^-16 (1 + |lse_i|).  The second term is the fp32 sum of up to 750 positive exponentials (round
-           to nearest: a random walk far below 2^-16 relative), at most a dozen rescales by exp(m_old - m_new) of 2^-22
-           each, and the log.
+``lse``    sum_j P_ij e_ij + 2^-16 (1 + |lse_i|).  The second term is the fp32 sum of up to S = 1025 positive exponentials,
+           the longest sequence the suite runs (the 512^2 ViT): each lane adds about S / 4 of them before a 4-lane
+           reduction, and round-to-nearest errors add like a random walk to about sqrt(S / 4) 2^-24 = 2^-20 relative; one
+           rescale by exp(m_old - m_new) per further 64-key block, at most 16 of 2^-22 each (2^-18); and the log.  The
+           total stays under 2^-17.5, so 2^-16 still holds at S = 1025.
 ``out``    2^-8 (P @ |V|) + sum_j P_ij (e_ij + dlse_i) (|v_j| + |o_i|) + tau (P @ |V|), then u_out |ref|.  P.V runs on bf16 P
            (2^-9 relative under round-to-nearest, doubled for margin, whatever the key blocking) while the denominator is
            summed from the unrounded fp32 values, so the rounding does not cancel.  A relative error d_j of P_ij moves
@@ -110,12 +113,34 @@ at 12608 rows, <= 10 + 32 steps in ``partial_reduce_kernel``), so tau = 2^-16 >=
 ``colsum``  sum of the given bf16 values: tau sum |y|.
 ``ln_fold``  Wg = bf16(fp32(W g)) is bit-exact; colsum = sum_k Wg (the rounded values): tau sum |Wg|; bias' = W beta + b:
            (tau + u) sum |W| |beta| + u (|bias'| + |b|).
-``l2_normalize_bwd``  dx = dy / |x| - x (x . dy) / |x|^3.  The fp32 norm is off by rel_n = (tau + 2u) / 2 + u relative,
+``l2_normalize_bwd``  dx = dy / |x| - x (x . dy) / |x|^3.  The fp32 norm is off by rel_n = (tau + 2u) / 2 + u relative
+           (``L2_NORM_REL``: tau for the sum of squares, then the sqrt's rounding),
            1 / |x| by rel_n + u; k = (x . dy) / |x|^3 by (tau + u) sum |x dy| / |x|^3 + |k| (3 rel_n + 4u); dx: |dy| / |x|
            (rel_n + 2u) + |x| dk + u (|x k| + |dx|).
 scatter-adds  (fp32 atomics, ``batch_sum``): onto init, count contributions in any order: (count + 1) u (|init| + sum |g|)
            per destination element.  ``window_scatter`` sums <= kw bf16 terms in a fixed order: kw u sum |terms|, then
            u_out |ref|.
+
+Embedding, gather, transpose and ranking kernels (``text_embed_ref`` and the functions after it)
+-------------------------------------------------------------------------------------------------
+``text_embed``, ``cls_row_init``, ``zero_padded_rows``, ``relpos_bias_build``, ``relpos_lut_build``, ``row_gather``,
+``relpos_bias_block``, ``transpose_bf16``, ``topk10_rows`` and ``recall_hits`` are exact: each output element is a gather,
+a copy, or one fp32 addition followed by at most one round-to-nearest to bf16.  The reference is the same fp32 operation in
+torch and the comparison is bit for bit.  One exception: ``text_embed`` zeroes pad rows, which the reference writes as
+(emb + pos) * (1 - mask); that can be -0.0, so pad rows are compared by value.
+``l2_normalize_rows``  y = x / max(|x|, 1e-12) in fp64.  The kernel's fp32 norm is off by ``L2_NORM_REL`` relative (as for
+           ``l2_normalize_bwd``: the sum of squares of a row is <= 16 + 5 + 8 additions deep per 256-thread CTA at D = 4096,
+           far under tau); max(., fp32(1e-12)) adds the rounding of 1e-12 to fp32 for a clamped row; the reciprocal and the
+           product add u each: |y| (L2_NORM_REL + rel(fp32(1e-12)) + 2u).  The bf16 copy is rounded from the same register,
+           so it equals bf16(y_fp32) bit for bit.
+``topk10_rows``  ranks each row by a total order (``order_key``): fp32 values in IEEE order with -0.0 equal to +0.0, every
+           NaN above +inf, -inf like any other value, and equal keys by the smaller column.  That is a stable descending
+           sort of the row, with NaN first as ``torch.topk`` ranks it.  Slots past C hold column -1 and value -inf.
+``topk_within``  for the retrieval similarity (bf16x3 GEMM logits, error dz = Z_TAU (|a| @ |b|^T)): the returned list is a
+           top-10 of some matrix within dz of the fp64 similarity.  Consecutive returned entries are ordered within their
+           two errors, and no column left out beats the 10th returned one by more than their two errors.  Recall@k can then
+           differ from the fp64 count only in rows whose k-th and (k+1)-th fp64 values lie within twice the row's largest
+           error (``recall_ref``).
 
 Optimizer (``adam_ref``, ``bf16_param_check``, ``grad_norm_ref``, ``clip_scale_ref``)
 -----------------------------------------------------------------------------------
@@ -553,6 +578,7 @@ GELU_REL = ERF_ABS / 2 + 4 * U32
 GELU_GRAD_ABS = ERF_ABS / 2 + 2.0 ** -21
 GELU_CURV = 0.8                 # max |gelu''(z)| = 2 phi(0) = 0.798
 RSQRT_REL = 2.0 ** -22
+L2_NORM_REL = (TAU + 2 * U32) / 2 + U32     # relative error of an fp32 row norm (sum of squares, then sqrt)
 
 
 def gelu_grad(z):
@@ -749,7 +775,7 @@ def l2_normalize_bwd_ref(x, dy):
     dot = (X * G).sum(1, keepdim=True)
     k = dot / nrm ** 3
     dx = G / nrm - X * k
-    rel_n = (TAU + 2 * U32) / 2 + U32
+    rel_n = L2_NORM_REL
     dk = (TAU + U32) * (X * G).abs().sum(1, keepdim=True) / nrm ** 3 + k.abs() * (3 * rel_n + 4 * U32)
     return dx, G.abs() / nrm * (rel_n + 2 * U32) + X.abs() * dk + U32 * ((X * k).abs() + dx.abs())
 
@@ -784,6 +810,127 @@ def window_scatter_ref(dwin, B, t_in, t_out, stride, kw, pad):
                 out[:, s] += v
                 mag[:, s] += v.abs()
     return out.reshape(B * t_in, groups * cg), kw * U32 * mag.reshape(B * t_in, groups * cg)
+
+
+# ----------------------------------------------------------------------------------------------------------------------
+# embedding, gather, transpose and ranking kernels (module docstring, "Embedding, gather, transpose and ranking kernels")
+# ----------------------------------------------------------------------------------------------------------------------
+def text_embed_ref(tokens, table, pos, cls, pad_idx):
+    """``opb_text_embed`` -> (x fp32 [B, T+1, D], pad uint8 [B, T+1]): row 0 = cls + pos[0], row s = fp32(table[tok]) +
+    pos[s], then (1 - pad) times that (pad rows may come out as -0.0)"""
+    B, T = tokens.shape
+    emb = torch.cat([cls.float().expand(B, 1, -1), table.float()[tokens]], 1)
+    pad = torch.cat([torch.zeros(B, 1, dtype=torch.bool, device=tokens.device), tokens == pad_idx], 1)
+    return (emb + pos[:T + 1].float()[None]) * (~pad)[..., None].float(), pad.to(torch.uint8)
+
+
+def relpos_bias_ref(table, bucket, S, s_pad):
+    """``opb_relpos_bias_build`` -> fp32 [H, S, s_pad]: table[bucket[i, j], h] for i, j < S, zero pad columns"""
+    H = table.shape[1]
+    out = torch.zeros(H, S, s_pad, dtype=torch.float32, device=table.device)
+    out[..., :S] = table[bucket[:S, :S]].permute(2, 0, 1)
+    return out
+
+
+def relpos_lut_ref(table, idx):
+    """``opb_relpos_lut_build`` -> fp32 [H, L]: lut[h, l] = table[idx[l], h]"""
+    return table[idx.long()].t()
+
+
+def row_gather_ref(src, idx, out_dtype, fill=None, add=None):
+    """``opb_row_gather``: out[r] = (src[idx[r]] if idx[r] >= 0 else fill, or 0) + add[r % period], one fp32 addition,
+    then rounded to out_dtype.  src [n, dim] (any row pitch), add fp32 [period, dim]."""
+    dim = src.shape[1]
+    base = torch.zeros(dim, dtype=torch.float32, device=src.device) if fill is None else fill.float()
+    v = torch.where((idx >= 0)[:, None], src.float()[idx.clamp_min(0)], base[None])
+    if add is not None:
+        a = add.reshape(-1, dim)
+        v = v + a[torch.arange(idx.numel(), device=src.device) % a.shape[0]]
+    return v.to(out_dtype)
+
+
+def relpos_bias_block_ref(table, bucket, ids, n, lo, canvas):
+    """``opb_relpos_bias_block`` on a copy of ``canvas`` [Bb, H, S, s_pad] -> (canvas, written mask):
+    canvas[bb, h, lo+i, lo+j] = table[bucket[p_i, p_j], h], p = ids[bb] (-1 -> n - 1) or arange(n)"""
+    Bb = canvas.shape[0]
+    p = ids.clone() if ids is not None else torch.arange(n, device=canvas.device).expand(Bb, n)
+    p = torch.where(p < 0, torch.full_like(p, n - 1), p)
+    out = canvas.clone()
+    out[:, :, lo:lo + n, lo:lo + n] = table[bucket[p[:, :, None], p[:, None, :]]].permute(0, 3, 1, 2)
+    written = torch.zeros(canvas.shape, dtype=torch.bool, device=canvas.device)
+    written[:, :, lo:lo + n, lo:lo + n] = True
+    return out, written
+
+
+def transpose_ref(x):
+    """``opb_transpose_bf16``: the [cols, rows] transpose of the logical [rows, cols] view, contiguous"""
+    return x.t().contiguous()
+
+
+def l2_normalize_ref(x):
+    """fp64 y = x / max(|x|, 1e-12) per row of fp32 x, and its bound (module docstring)"""
+    X = x.double()
+    y = X / X.norm(dim=1, keepdim=True).clamp_min(1e-12)
+    return y, y.abs() * (L2_NORM_REL + f32_rel(1e-12) + 2 * U32)
+
+
+def order_key(x):
+    """int64 key of the order ``topk10_rows`` ranks fp32 values by, unique per column of x [R, C]: fp32 IEEE order with
+    -0.0 == +0.0, every NaN above +inf, and among equal values the smaller column first (the larger key)"""
+    b = x.float().contiguous().view(torch.int32).long() & 0xFFFFFFFF
+    k = torch.where(b >= 2 ** 31, 0xFFFFFFFF - b, b | 2 ** 31)
+    k = torch.where(x == 0, torch.full_like(k, 2 ** 31), k)
+    k = torch.where(torch.isnan(x), torch.full_like(k, 0xFFFFFFFF), k)
+    col = torch.arange(x.shape[1], device=x.device)
+    return (k - 2 ** 31) * 2 ** 32 + (2 ** 31 - 1 - col)
+
+
+def topk10_ref(x):
+    """top-10 of every row of fp32 x [R, C] in the order of ``order_key`` (a stable descending sort, NaN first) ->
+    (idx int32 [R, 10], val fp32 [R, 10]); slots past C hold -1 and -inf.  The keys are unique, so torch.topk of them has no
+    tie to break."""
+    R, C = x.shape
+    k = min(10, C)
+    top = order_key(x).topk(k, dim=1).indices
+    idx = torch.full((R, 10), -1, dtype=torch.int64, device=x.device)
+    val = torch.full((R, 10), float("-inf"), dtype=torch.float32, device=x.device)
+    idx[:, :k] = top
+    val[:, :k] = x.gather(1, top)
+    return idx.int(), val
+
+
+def recall_hits_ref(idx, cand_ids, row_ids):
+    """``opb_recall_hits`` -> [hits@1, hits@5, hits@10]: rows whose id is among the ids of their first 1 / 5 / 10 ranked
+    candidates (column -1 never hits)"""
+    g = idx.long()
+    ids = torch.where(g >= 0, cand_ids[g.clamp_min(0)], torch.full_like(g, -2 ** 62))
+    eq = ids == row_ids[:, None]
+    return [int(eq[:, :k].any(1).sum()) for k in (1, 5, 10)]
+
+
+def topk_within(z, dz, idx):
+    """Rows whose returned list ``idx`` [R, 10] is a top-10 of some matrix within ``dz`` of the fp64 similarity z [R, C]
+    (``argmax_ok`` for a ranked list): ten distinct columns in range, each returned entry no smaller than the next one
+    minus both their errors, and no column left out above the 10th returned one by more than both their errors."""
+    R, C = z.shape
+    g = idx.long()
+    valid = ((g >= 0) & (g < C)).all(1) & (g.sort(1).values.diff(dim=1) != 0).all(1)
+    g = g.clamp(0, C - 1)
+    zi, di = z.gather(1, g), dz.gather(1, g)
+    ordered = (zi[:, :-1] >= zi[:, 1:] - di[:, :-1] - di[:, 1:]).all(1)
+    left_out = torch.ones(R, C, dtype=torch.bool, device=z.device).scatter_(1, g, False)
+    beats = left_out & (z > zi[:, -1:] + dz + di[:, -1:])
+    return valid & ordered & ~beats.any(1)
+
+
+def recall_ref(z, dz, cand_ids, row_ids):
+    """fp64 Recall@{1,5,10} hit counts of the similarity z [R, C >= 11] and, per k, the number of rows whose k-th and
+    (k+1)-th largest values lie within twice the row's largest error, the only rows whose hit can differ"""
+    top = z.topk(11, dim=1)
+    hits = recall_hits_ref(top.indices[:, :10], cand_ids, row_ids)
+    margin = 2 * dz.max(1).values
+    near = [int((top.values[:, k - 1] - top.values[:, k] <= margin).sum()) for k in (1, 5, 10)]
+    return hits, near
 
 
 # ----------------------------------------------------------------------------------------------------------------------

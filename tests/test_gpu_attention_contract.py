@@ -141,18 +141,19 @@ def run_dense(K, qkv, table, kp, B, S, H):
 
 
 FWD_S = [2, 17, 63, 64, 65, 197, 224, 225, 257, 321, 384, 385, 750]
+VIT_S = [577, 785, 1025]            # the 384^2, 448^2 and 512^2 ViTs (w = 24, 28, 32): dense tables only
 
 
 @pytest.mark.parametrize("bias_kind", ["normal", "stress"])
 @pytest.mark.parametrize("pad", ["none", "right"])
-@pytest.mark.parametrize("S", FWD_S)
+@pytest.mark.parametrize("S", FWD_S + VIT_S)
 def test_forward_dense(K, ratios, S, pad, bias_kind):
     """shared table; the same table replicated per sample must give the same bits"""
     B, H = 3, 2
     g = seed("dense", S, pad, bias_kind)
     qkv, kp = make_qkv(B, S, H, g), key_pad(B, S, pad)
     bias = make_bias((H, S, S), S, bias_kind, g)
-    table = dense_table(bias, s_pad_for(S, FWD_S.index(S)))
+    table = dense_table(bias, s_pad_for(S, (FWD_S + VIT_S).index(S)))
     got = run_dense(K, qkv, table, kp, B, S, H)
     check_fwd(ratios, f"dense {bias_kind}", got, R.attention_ref(qkv, bias, kp, B, S, H), B, S, H)
     rep = table[None].repeat(B, 1, 1, 1).contiguous()
@@ -248,6 +249,18 @@ def test_forward_production_shape(K, ratios, form):
     check_fwd(ratios, f"{form} B=64 H=24", got, R.attention_ref(qkv, dense, None, B, S, H), B, S, H)
 
 
+def test_forward_vit_512_shape(K, ratios):
+    """the 512^2 ViT shape (one_piece_g_512): B = 1, S = 1025, H = 24, the dense table of the w = 32 image buckets"""
+    import restated
+    B, S, H, w = 1, 1025, 24, 32
+    g = seed("vit 512")
+    qkv = make_qkv(B, S, H, g)
+    table = torch.randn((2 * w - 1) ** 2 + 3, H, device="cuda", generator=g)
+    bias = table[restated.make_image_bucket_position(w).cuda()].permute(2, 0, 1).contiguous()
+    got = run_dense(K, qkv, dense_table(bias, s_pad_for(S, 1)), None, B, S, H)
+    check_fwd(ratios, "dense B=1 H=24 S=1025", got, R.attention_ref(qkv, bias, None, B, S, H), B, S, H)
+
+
 # --------------------------------------------------------------------------------------------------------------------
 # backward
 # --------------------------------------------------------------------------------------------------------------------
@@ -300,7 +313,7 @@ def bwd_dense_case(K, ratios, family, B, S, H, bias, table, kp, g):
 
 
 @pytest.mark.parametrize("bias_kind", ["normal", "stress"])
-@pytest.mark.parametrize("S", [17, 65, 197, 225, 385, 750])
+@pytest.mark.parametrize("S", [17, 65, 197, 225, 385, 750] + VIT_S)
 def test_backward_dense(K, ratios, S, bias_kind):
     """shared table; the same table replicated per sample must give the same dqkv bits"""
     B, H = 3, 2

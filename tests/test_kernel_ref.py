@@ -1,7 +1,11 @@
 """CPU: the fp64 reference and per-element bounds of tests/kernel_ref.py.  A correct kernel, emulated here in fp32 (bf16
 operands, fp32 matmul, the epilogue and the LayerNorm statistics in fp32 as the kernel evaluates them; for attention the
 blocked online soft-max and the recomputing backward), must pass the bounds; each of the subtle mistakes a GEMM, InfoNCE
-or attention kernel can make must fail them."""
+or attention kernel can make must fail them.  The exact kernels (top-10 ranking, transpose, row gather, block bias) are
+ported or emulated and must equal their references bit for bit, and their planted mistakes must not."""
+import struct
+
+import numpy as np
 import pytest
 import torch
 
@@ -1004,3 +1008,286 @@ def test_clip_scale_keeps_nan_and_zeroes_inf():
     assert math.isnan(R.clip_scale_ref(float("nan"), 0.0, 1.0, 1.0)[0])
     assert R.clip_scale_ref(float("inf"), 0.0, 0.5, 1.0)[0] == 0.0
     assert R.clip_scale_ref(3.0, 0.0, 0.5, 0.0) == (0.5, 0.0)
+
+
+# ----------------------------------------------------------------------------------------------------------------------
+# embedding, gather, transpose and ranking kernels
+# ----------------------------------------------------------------------------------------------------------------------
+def _key32(x):
+    """order key of one fp32 value (``order_key`` of csrc/recall.cu)"""
+    if x != x:
+        return 0xFFFFFFFF
+    if x == 0:
+        return 0x80000000
+    u = struct.unpack("<I", struct.pack("<f", x))[0]
+    return (~u & 0xFFFFFFFF) if u >> 31 else u | 0x80000000
+
+
+def topk10_warp(flat, ld, rows, C, mutation=None):
+    """Python port of ``topk_rows_kernel`` on a flat fp32 buffer of row pitch ld: 32 lane lists of strided columns, then 10
+    arg-max merge rounds.  Mutations: 'strict_gt_neg_inf' (float lists initialised to -inf, an entry inserted only when
+    strictly greater than the last one: the rule before the total order), 'ties_to_larger_index', 'ignore_ld'."""
+    vals, none = flat.tolist(), 0x7FFFFFFF
+    out = []
+    for r in range(rows):
+        base = r * (C if mutation == "ignore_ld" else ld)
+        lanes = []
+        for lane in range(32):
+            if mutation == "strict_gt_neg_inf":
+                t = [(float("-inf"), -none)] * 10                  # (value, -column): larger is better
+                for c in range(lane, C, 32):
+                    x = vals[base + c]
+                    if x > t[9][0]:
+                        t[9] = (x, -c)
+                        for i in range(9, 0, -1):
+                            if t[i][0] > t[i - 1][0]:
+                                t[i], t[i - 1] = t[i - 1], t[i]
+            else:
+                t = [0] * 10
+                for c in range(lane, C, 32):
+                    low, k = (c if mutation == "ties_to_larger_index" else ~c & 0xFFFFFFFF), _key32(vals[base + c])
+                    if k > t[9] >> 32 or (mutation == "ties_to_larger_index" and k == t[9] >> 32):
+                        t[9] = k << 32 | low
+                        for i in range(9, 0, -1):
+                            if t[i] > t[i - 1]:
+                                t[i], t[i - 1] = t[i - 1], t[i]
+            lanes.append(t)
+        row = []
+        for _ in range(10):
+            if mutation == "strict_gt_neg_inf":
+                best = max(lanes, key=lambda t: (t[0][0], t[0][1]))[0]
+                row.append(-1 if best[1] == -none else -best[1])
+                if best[1] != -none:
+                    w = next(t for t in lanes if t[0] == best)
+                    w[:] = w[1:] + [(float("-inf"), -none)]
+                continue
+            best = max(t[0] for t in lanes)
+            low = best & 0xFFFFFFFF
+            row.append(-1 if best == 0 else (low if mutation == "ties_to_larger_index" else ~low & 0xFFFFFFFF))
+            if best:
+                w = next(t for t in lanes if t[0] == best)
+                w[:] = w[1:] + [0]
+        out.append(row)
+    return torch.tensor(out, dtype=torch.int32)
+
+
+def _topk_rows(C, ld):
+    """rows for the top-10 port, in a buffer of pitch ld whose gap holds NaN (which would rank first if read): ties within a
+    lane (columns c and c + 32) and across lanes, -inf, NaN of both signs, signed zeros, an all-equal row, an all -inf row,
+    an all-NaN row, fewer than 10 entries above -inf"""
+    g = torch.Generator().manual_seed(C)
+    x = torch.tensor([-1.0, 0.0, 0.5, 2.0])[torch.randint(0, 4, (14, C), generator=g)]
+    if C > 32:
+        x[0, 32:] = x[0, :C - 32].clone()                                # column c + 32 equals column c: a tie within a lane
+    x[1] = 0.5
+    x[2] = float("-inf")
+    x[3] = float("nan")
+    x[4] = float("-inf")
+    x[4, ::9] = 1.0
+    x[5, ::3] = float("-inf")
+    x[5, 1::4] = float("nan")
+    x[6, ::2] = -0.0
+    x[6, 1::3] = float("-inf")
+    x[7].view(torch.int32)[::4] = 0xFFC00001 - 2 ** 32            # negative NaN
+    x[8, ::2] = float("inf")
+    buf = torch.full((x.shape[0], ld), float("nan"))
+    buf[:, :C] = x
+    return x, buf.view(-1)
+
+
+@pytest.mark.parametrize("C", [1, 7, 10, 31, 33, 70])
+def test_topk10_port_is_the_total_order(C):
+    x, flat = _topk_rows(C, C + 3)
+    want = R.topk10_ref(x)[0]
+    assert torch.equal(topk10_warp(flat, C + 3, x.shape[0], C), want)
+    finite = torch.isfinite(x).all(1)
+    tv, ti = x[finite].topk(min(10, C), dim=1, sorted=True)
+    assert torch.equal(R.topk10_ref(x)[1][finite][:, :min(10, C)], tv)
+
+
+def test_topk10_reference_ranks_like_torch():
+    """NaN first, then values, -inf like any other value, ties by the smaller column: torch.sort(stable) on the CPU"""
+    x = torch.tensor([[1.0, float("nan"), float("-inf"), 2.0, float("-inf"), 0.5, 2.0, float("nan"), -0.0, 0.0, -1.0, 0.5]])
+    i, v = R.topk10_ref(x)
+    s = torch.sort(x, dim=1, descending=True, stable=True).indices[:, :10]
+    assert i.tolist() == [[1, 7, 3, 6, 0, 5, 11, 8, 9, 10]] and torch.equal(i.long(), s)
+    assert torch.isnan(v[0, :2]).all() and v[0, 2:].tolist() == [2.0, 2.0, 1.0, 0.5, 0.5, -0.0, 0.0, -1.0]
+    i3, v3 = R.topk10_ref(x[:, :3])
+    assert i3.tolist() == [[1, 0, 2] + [-1] * 7] and v3[0, 3:].eq(float("-inf")).all()
+
+
+@pytest.mark.parametrize("mutation", ["strict_gt_neg_inf", "ties_to_larger_index", "ignore_ld"])
+def test_topk10_mutation_fails(mutation):
+    """each mistake returns a wrong column on some rows; the earlier strict-> rule exactly on the rows holding -inf or NaN
+    (run with -s to see the counts)"""
+    C = 70
+    x, flat = _topk_rows(C, C + 3)
+    want = R.topk10_ref(x)[0]
+    bad = (topk10_warp(flat, C + 3, x.shape[0], C, mutation) != want).any(1)
+    print(f"{mutation}: {int(bad.sum())} of {x.shape[0]} rows wrong")
+    assert bad.sum() >= 3
+    if mutation == "strict_gt_neg_inf":
+        special = (torch.isnan(x) | (x == float("-inf"))).any(1)
+        assert torch.equal(bad, special & bad) and bad[[2, 3, 4]].all()
+
+
+def emulate_l2_normalize(x, mutation=None):
+    """``l2_normalize_kernel`` in fp32: 256 threads, thread t adds x[c]^2 for c = t, t + 256, ...; a butterfly over each
+    warp; lane 0 of warp 0 adds the 8 warp partials in order; y = x * (1 / max(sqrt(s), 1e-12)).  Mutations: 'no_clamp',
+    'sum_in_bf16' (squares and partial sums rounded to bf16)."""
+    rows, D = x.shape
+    xs = x.float()
+    sq = torch.nn.functional.pad(xs * xs, (0, (-D) % 256)).view(rows, -1, 256)
+    rnd = (lambda t: t.bfloat16().float()) if mutation == "sum_in_bf16" else (lambda t: t)
+    part = torch.zeros(rows, 256)
+    for s in range(sq.shape[1]):
+        part = rnd(part + rnd(sq[:, s]))
+    w = part.view(rows, 8, 32)
+    lane = torch.arange(32)
+    for o in (16, 8, 4, 2, 1):
+        w = rnd(w + w[:, :, lane ^ o])
+    tot = torch.zeros(rows)
+    for i in range(8):
+        tot = rnd(tot + w[:, i, 0])
+    nrm = torch.sqrt(tot)
+    inv = 1.0 / (nrm if mutation == "no_clamp" else torch.clamp_min(nrm, float(np.float32(1e-12))))
+    return xs * inv[:, None]
+
+
+def _l2_rows(D):
+    g = torch.Generator().manual_seed(D)
+    x = torch.randn(8, D, generator=g) * (0.5 + torch.rand(8, 1, generator=g))
+    x[1] *= 1e6
+    x[2] *= 1e-6
+    x[3] = 0.0
+    x[4] *= 1e-15
+    x[5] = 0.0
+    x[5, D // 2] = 3.7
+    return x
+
+
+@pytest.mark.parametrize("D", [1, 31, 257, 1536, 4096])
+def test_l2_normalize_emulation_passes(D):
+    x = _l2_rows(D)
+    y = emulate_l2_normalize(x)
+    ref, bound = R.l2_normalize_ref(x)
+    r = R.assert_within(y, ref, bound, 1.0, torch.float32, what=f"l2_normalize D={D}")
+    print(f"l2_normalize D={D}: {r:.3g} of the bound")
+    assert y[3].eq(0).all() and not torch.isnan(y).any()
+
+
+@pytest.mark.parametrize("mutation", ["no_clamp", "sum_in_bf16"])
+def test_l2_normalize_mutation_fails(mutation):
+    x = _l2_rows(1536)
+    ref, bound = R.l2_normalize_ref(x)
+    r = _ratio(emulate_l2_normalize(x, mutation), ref, bound, torch.float32)
+    print(f"{mutation}: exceeds its bound {r:.3g}-fold")
+    assert r >= 10
+
+
+def emulate_transpose(x, mutation=None):
+    """``transpose_bf16_vec_kernel``: 64 x 64 tiles staged in shared memory as tile[col][row]; 'tile_swapped' writes the
+    staged tile back as tile[row][col]"""
+    rows, cols = x.shape
+    out = torch.empty(cols, rows, dtype=x.dtype)
+    for r0 in range(0, rows, 64):
+        for c0 in range(0, cols, 64):
+            blk = x[r0:r0 + 64, c0:c0 + 64]
+            tile = torch.zeros(64, 64, dtype=x.dtype)
+            tile[:blk.shape[1], :blk.shape[0]] = blk.t()
+            if mutation == "tile_swapped":
+                tile = tile.t()
+            out[c0:c0 + 64, r0:r0 + 64] = tile[:min(64, cols - c0), :min(64, rows - r0)]
+    return out
+
+
+def emulate_row_gather(src, idx, fill, add, out_dtype, mutation=None):
+    """``row_gather_kernel`` row by row; 'add_period_off_by_one' takes the addend row r % (period - 1)"""
+    period = add.shape[0] - (1 if mutation == "add_period_off_by_one" else 0)
+    rows = []
+    for r, s in enumerate(idx.tolist()):
+        v = src[s].float() if s >= 0 else fill
+        rows.append(v + add[r % period])
+    return torch.stack(rows).to(out_dtype)
+
+
+def emulate_bias_block(table, bucket, ids, n, lo, canvas, mutation=None):
+    """``relpos_bias_block_kernel`` on the flat canvas; 'cols_without_lo' writes block row i at columns j instead of lo + j,
+    'pad_id_to_0' maps -1 ids to 0 instead of n - 1"""
+    out = canvas.clone()
+    Bb, H, S, s_pad = canvas.shape
+    flat = out.view(-1)
+    fix = 0 if mutation == "pad_id_to_0" else n - 1
+    for bb in range(Bb):
+        p = [fix if q < 0 else q for q in ids[bb].tolist()]
+        for i in range(n):
+            base = (bb * H * S + lo + i) * s_pad + (0 if mutation == "cols_without_lo" else lo)
+            for j in range(n):
+                for h in range(H):
+                    flat[base + h * S * s_pad + j] = table[bucket[p[i], p[j]], h]
+    return out
+
+
+def _exact_cases(mutation=None):
+    """(got, want) pairs of the exact kernels' emulations"""
+    g = torch.Generator().manual_seed(31)
+    x = torch.randn(130, 200, generator=g).bfloat16()
+    src = torch.randn(40, 12, generator=g).bfloat16()
+    idx = torch.randint(-1, 40, (23,), generator=g)
+    fill, add = torch.randn(12, generator=g), torch.randn(5, 12, generator=g)
+    table, bucket = torch.randn(50, 3, generator=g), torch.randint(0, 50, (30, 30), generator=g)
+    ids = torch.randint(0, 30, (2, 9), generator=g)
+    ids[:, -2:] = -1
+    canvas = torch.full((2, 3, 14, 16), float("nan"))
+    return {"transpose": (emulate_transpose(x, mutation), R.transpose_ref(x)),
+            "row_gather": (emulate_row_gather(src, idx, fill, add, torch.bfloat16, mutation),
+                           R.row_gather_ref(src, idx, torch.bfloat16, fill, add)),
+            "bias_block": (emulate_bias_block(table, bucket, ids, 9, 4, canvas, mutation),
+                           R.relpos_bias_block_ref(table, bucket, ids, 9, 4, canvas)[0])}
+
+
+def _same_bits(a, b):
+    it = torch.int16 if a.dtype == torch.bfloat16 else torch.int32
+    return a.shape == b.shape and torch.equal(a.view(it), b.view(it))
+
+
+def test_exact_emulations_match_references():
+    for name, (got, want) in _exact_cases().items():
+        assert _same_bits(got, want), name
+
+
+@pytest.mark.parametrize("mutation,kernel", [("tile_swapped", "transpose"), ("add_period_off_by_one", "row_gather"),
+                                             ("cols_without_lo", "bias_block"), ("pad_id_to_0", "bias_block")])
+def test_exact_mutation_fails(mutation, kernel):
+    got, want = _exact_cases(mutation)[kernel]
+    assert not _same_bits(got, want), mutation
+
+
+def test_topk_within_and_recall_bounds():
+    """an fp32 similarity ranked by the total order passes ``topk_within`` against the fp64 one, and its Recall@k lies within
+    the near-tie rows; a list with its 1st and 10th entries swapped, or with the 11th entry in place of the 10th where the
+    gap is wide, fails"""
+    g = torch.Generator().manual_seed(37)
+    a = torch.nn.functional.normalize(torch.randn(60, 64, generator=g), dim=1)
+    b = torch.nn.functional.normalize(torch.randn(90, 64, generator=g), dim=1)
+    b[1] = b[0] + 1e-7                                             # near-duplicate candidates
+    z = a.double() @ b.double().t()
+    dz = R.Z_TAU * (a.double().abs() @ b.double().abs().t())
+    sim = a @ b.t()
+    idx = R.topk10_ref(sim)[0]
+    assert R.topk_within(z, dz, idx).all()
+    cand, own = torch.randint(0, 30, (90,), generator=g), torch.randint(0, 30, (60,), generator=g)
+    hits, near = R.recall_ref(z, dz, cand, own)
+    got = R.recall_hits_ref(idx, cand, own)
+    assert all(abs(x - y) <= n for x, y, n in zip(got, hits, near))
+    swapped = idx.clone()
+    swapped[:, [0, 9]] = swapped[:, [9, 0]]
+    assert not R.topk_within(z, dz, swapped).any()
+    full = z.topk(11, dim=1).indices
+    wide = (z.gather(1, full[:, 9:10]) - z.gather(1, full[:, 10:11]) > 1e-3).squeeze(1)
+    eleventh = idx.clone().long()
+    eleventh[:, 9] = full[:, 10]
+    assert not R.topk_within(z, dz, eleventh)[wide].any() and wide.sum() > 30
+    dup = idx.clone()
+    dup[:, 9] = dup[:, 8]
+    assert not R.topk_within(z, dz, dup).any()

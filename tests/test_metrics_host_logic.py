@@ -1,7 +1,7 @@
 """CPU: the fp64 restatement of the classification metrics (tests/metrics_ref.py) against the reference's own Accuracy and MAP
 (tests/golden/metrics.pt, made by oracle/make_golden_metrics.py) and against scikit-learn when it is importable; seven planted
 mistakes, each of which must exceed a bound at least 100-fold or change an exact count; the distributed exchange of
-merge_results over gloo with uneven shards; and the metric names."""
+merge_results over gloo with uneven shards; the metric names; and Recall's refusal of fewer than 10 candidates."""
 import os
 import socket
 
@@ -208,3 +208,15 @@ def test_metric_names_and_protocol():
     for cls in (Accuracy, MAP):
         for name in ("initialize", "compute", "merge_results"):
             assert callable(getattr(cls, name))
+
+
+@pytest.mark.parametrize("n_img,n_txt", [(9, 40), (40, 9), (3, 3)])
+def test_recall_refuses_fewer_than_10_candidates(n_img, n_txt):
+    """Recall@10 with fewer than 10 candidates in either direction raises (the reference's topk(k=10) does), naming the
+    counts, instead of returning padded predictions; nothing reaches a kernel"""
+    from one_peace_b200.metrics import Recall
+    rec = Recall()
+    rec.initialize(torch.arange(n_txt), torch.randn(n_txt, 8))
+    rec.compute(torch.arange(n_img), torch.randn(n_img, 8))
+    with pytest.raises(RuntimeError, match=f"got {n_txt} texts and {n_img} images"):
+        rec.merge_results(output_predict=True)
