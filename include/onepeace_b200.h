@@ -118,6 +118,28 @@ int opb_attention_tc_fwd(const void* qkv, const float* lut, const float* lut_max
 int opb_relpos_lut_build(const float* table, const int32_t* idx, float* lut, int L, int H, void* stream);
 
 /*
+ * Decomposed relative position of the detection backbone (one_peace_vision/det/models/onepeace.py:204-207, detectron2's
+ * add_decomposed_rel_pos), on a kh x kw grid of S = kh * kw tokens per sequence, head_dim 64.
+ *   opb_relpos_decomp_proj : rel_h fp32 [B, H, S, kh], rel_w fp32 [B, H, S, kw] with
+ *       rel_h[b][h][i][ky] = q . rel_pos_h[pos_y[i] - ky + kh - 1],  rel_w[b][h][i][kx] = q . rel_pos_w[pos_x[i] - kx + kw - 1]
+ *     where q = q_unscale * qkv[b * S + i, h * 64 : h * 64 + 64] (the bf16 q columns carry head_dim^-0.5; the reference
+ *     uses the unscaled q, so q_unscale = 8).  rel_pos_h fp32 [2 kh - 1, 64], rel_pos_w fp32 [2 kw - 1, 64]; pos_y / pos_x
+ *     int32 [S] the grid position of each row (any row order).  fp32 products, summed over the 64 channels in order.
+ *   opb_attention_decomp_fwd : opb_attention_tc_fwd's LUT-form attention (no key padding, no seg_split) with
+ *     rel_h[b][h][i][key_y[j]] + rel_w[b][h][i][key_x[j]] added to logit (i, j) after the LUT bias; key_y / key_x int32
+ *     [S] the key grid coordinates.  out / lse / ln_stats as in opb_attention_fwd (lse and ln_stats may be NULL).
+ * Both need kh * kw == S and 1 <= kh, kw <= 256.  A row position or key coordinate outside the grid yields NaN in the
+ * terms or logits it touches (never an out-of-bounds read).
+ */
+int opb_relpos_decomp_proj(const void* qkv, const float* rel_pos_h, const float* rel_pos_w, const int32_t* pos_y,
+                           const int32_t* pos_x, float q_unscale, float* rel_h, float* rel_w, int B, int S, int H, int kh,
+                           int kw, void* stream);
+int opb_attention_decomp_fwd(const void* qkv, const float* lut, int lut_len, const int32_t* code_row,
+                             const int32_t* code_col, const float* rel_h, const float* rel_w, const int32_t* key_y,
+                             const int32_t* key_x, int kh, int kw, void* out, float* lse, float* ln_stats, int B, int S,
+                             int H, void* stream);
+
+/*
  * GEMM with the full epilogue description (superset of opb_gemm_bf16).  Adds the fused-LayerNorm form
  *   LN(x) W^T + b  =  rstd[m] * (acc - mu[m] * colsum[n]) + bias'[n]
  * where A holds the UN-normalised rows (bf16), B = W * diag(ln_weight) (bf16), colsum[n] = sum_k B[n,k],

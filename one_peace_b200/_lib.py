@@ -29,6 +29,10 @@ SIGNATURES = {
     "opb_attention_tc_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                      c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
     "opb_relpos_lut_build": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p]),
+    "opb_relpos_decomp_proj": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_float, c_void_p, c_void_p, c_int,
+                                       c_int, c_int, c_int, c_int, c_void_p]),
+    "opb_attention_decomp_fwd": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                         c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
     "opb_gemm_bf16_ex": (c_int, [c_void_p, c_void_p]),
     "opb_row_stats_cast": (c_int, [c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_void_p, c_int, c_int, c_float, c_void_p]),
     "opb_ln_stats_finalize": (c_int, [c_void_p, c_int, c_int, c_int, c_float, c_void_p, c_void_p, c_void_p]),

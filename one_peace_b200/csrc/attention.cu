@@ -62,13 +62,25 @@ OPB_DEVICE float lut_bias(const LutBias& lb, const float* lut_h, int crow, int q
   return lut_h[crow - lb.code_col[key]];
 }
 
+// Decomposed relative position (detectron2 add_decomposed_rel_pos, det/models/onepeace.py:204-207): logit (i, j) gains
+// rel_h[b][h][i][key_y[j]] + rel_w[b][h][i][key_x[j]].  kDecomp kernels stage the query tile's rel_h | rel_w rows
+// (pitch kh + kw + 1 floats, odd against bank conflicts) after AttnSmem, and each key block's packed coordinates
+// (ky | kx << 16) in kc.  A coordinate outside [0, kh) / [0, kw) makes its logit NaN instead of reading out of bounds.
+struct DecompSmem {
+  int kc[2][kKTile];
+  float rel[kQTile][1];   // [kQTile][kh + kw + 1]
+};
+
+template <bool kDecomp>
 __global__ void __launch_bounds__(128, 4)
 attention_fwd_kernel(const __nv_bfloat16* __restrict__ qkv, const float* __restrict__ bias,
                      const uint8_t* __restrict__ key_pad, __nv_bfloat16* __restrict__ out, float* __restrict__ lse,
                      float* __restrict__ ln_stats, int B, int S, int H, int s_pad, long bias_bstride,
-                     const LutBias lb) {
+                     const LutBias lb, const DecompRel dr) {
   extern __shared__ __align__(16) uint8_t attn_smem_raw[];
   AttnSmem& sm = *reinterpret_cast<AttnSmem*>(attn_smem_raw);
+  DecompSmem& ds = *reinterpret_cast<DecompSmem*>(attn_smem_raw + sizeof(AttnSmem));
+  const int rel_pitch = dr.kh + dr.kw + 1;
 
   const int q_chunks = (S + kQTile - 1) / kQTile;
   const int chunk = blockIdx.x % q_chunks;
@@ -112,7 +124,25 @@ attention_fwd_kernel(const __nv_bfloat16* __restrict__ qkv, const float* __restr
       cp_async16(&sm.k[buf][r][c], kbase + off, ok);
       cp_async16(&sm.v[buf][r][c], vbase + off, ok);
     }
+    if constexpr (kDecomp) {
+      // buf was last read before the previous block's closing __syncthreads; read after the next block's first one
+      if (tid < kKTile) {
+        const int key = k0 + tid;
+        const int y = key < S ? dr.key_y[key] : 0, x = key < S ? dr.key_x[key] : 0;
+        ds.kc[buf][tid] = static_cast<unsigned>(y) < static_cast<unsigned>(dr.kh) &&
+                          static_cast<unsigned>(x) < static_cast<unsigned>(dr.kw) ? y | (x << 16) : -1;
+      }
+    }
   };
+  if constexpr (kDecomp) {
+    const float* rh = dr.rel_h + (static_cast<long>(b) * H + h) * S * dr.kh;
+    const float* rw = dr.rel_w + (static_cast<long>(b) * H + h) * S * dr.kw;
+    for (int r = warp; r < kQTile; r += 4) {
+      const int q = q0 + r < S ? q0 + r : S - 1;
+      for (int c = lane; c < dr.kh; c += 32) ds.rel[0][r * rel_pitch + c] = rh[static_cast<long>(q) * dr.kh + c];
+      for (int c = lane; c < dr.kw; c += 32) ds.rel[0][r * rel_pitch + dr.kh + c] = rw[static_cast<long>(q) * dr.kw + c];
+    }
+  }
   load_kv(0, 0);
   cp_async_commit();
 
@@ -177,10 +207,24 @@ attention_fwd_kernel(const __nv_bfloat16* __restrict__ qkv, const float* __restr
         }
         const bool dead0 = (key >= S) || (kp != nullptr && kp[key] != 0);
         const bool dead1 = (key + 1 >= S) || (kp != nullptr && kp[key + 1] != 0);
-        s[nt][0] = dead0 ? -INFINITY : s[nt][0] + b00;
-        s[nt][1] = dead1 ? -INFINITY : s[nt][1] + b01;
-        s[nt][2] = dead0 ? -INFINITY : s[nt][2] + b10;
-        s[nt][3] = dead1 ? -INFINITY : s[nt][3] + b11;
+        if constexpr (kDecomp) {
+          // ((q.k + bias) + rel_h) + rel_w, the reference's order of fp32 adds
+          const int2 kc = *reinterpret_cast<const int2*>(&ds.kc[buf][nt * 8 + 2 * t]);
+          auto add = [&](float v, int row, int c) {
+            const float* r = &ds.rel[0][row * rel_pitch];
+            return c >= 0 ? (v + r[c & 0xffff]) + r[dr.kh + (c >> 16)] : NAN;
+          };
+          const int rlo = warp * 16 + g;
+          s[nt][0] = dead0 ? -INFINITY : add(s[nt][0] + b00, rlo, kc.x);
+          s[nt][1] = dead1 ? -INFINITY : add(s[nt][1] + b01, rlo, kc.y);
+          s[nt][2] = dead0 ? -INFINITY : add(s[nt][2] + b10, rlo + 8, kc.x);
+          s[nt][3] = dead1 ? -INFINITY : add(s[nt][3] + b11, rlo + 8, kc.y);
+        } else {
+          s[nt][0] = dead0 ? -INFINITY : s[nt][0] + b00;
+          s[nt][1] = dead1 ? -INFINITY : s[nt][1] + b01;
+          s[nt][2] = dead0 ? -INFINITY : s[nt][2] + b10;
+          s[nt][3] = dead1 ? -INFINITY : s[nt][3] + b11;
+        }
       }
 
       // ---- online softmax (rows g and g+8 of this warp's 16) ----
@@ -292,9 +336,9 @@ static int launch_fwd(const void* qkv, const float* bias, const uint8_t* key_pad
     return attention_fwd_short(qkv, bias, key_pad, out, lse, ln_stats, B, S, H, s_pad, bias_bstride, lb, stream);
   const int q_chunks = (S + kQTile - 1) / kQTile;
   const long grid = static_cast<long>(H) * q_chunks * B;
-  attention_fwd_kernel<<<static_cast<unsigned>(grid), 128, sizeof(AttnSmem), stream>>>(
+  attention_fwd_kernel<false><<<static_cast<unsigned>(grid), 128, sizeof(AttnSmem), stream>>>(
       reinterpret_cast<const __nv_bfloat16*>(qkv), bias, key_pad, reinterpret_cast<__nv_bfloat16*>(out), lse, ln_stats,
-      B, S, H, s_pad, bias_bstride, lb);
+      B, S, H, s_pad, bias_bstride, lb, DecompRel());
   return cudaGetLastError() == cudaSuccess ? OPB_OK : OPB_ERR_CUDA;
 }
 
@@ -312,6 +356,31 @@ int attention_lut_fwd(const void* qkv, const float* lut, int lut_len, const int*
   LutBias lb;
   lb.lut = lut; lb.lut_len = lut_len; lb.code_row = code_row; lb.code_col = code_col; lb.seg_split = seg_split;
   return launch_fwd(qkv, nullptr, key_pad, out, lse, ln_stats, B, S, H, 0, 0, lb, stream);
+}
+
+// The LUT-form kernel plus the decomposed relative-position terms, for any S (no wgmma short path).  The rel_h / rel_w
+// rows of a 64-query tile take 64 * (kh + kw + 1) floats of shared memory on top of AttnSmem.
+int attention_decomp_fwd(const void* qkv, const float* lut, int lut_len, const int* code_row, const int* code_col,
+                         const DecompRel& dr, void* out, float* lse, float* ln_stats, int B, int S, int H,
+                         cudaStream_t stream) {
+  if (B <= 0 || S <= 0 || H <= 0 || lut_len <= 0 || dr.kh <= 0 || dr.kw <= 0) return OPB_ERR_INVALID;
+  if (static_cast<long>(dr.kh) * dr.kw != S || dr.kh > kDecompMaxK || dr.kw > kDecompMaxK) return OPB_ERR_INVALID;
+  LutBias lb;
+  lb.lut = lut; lb.lut_len = lut_len; lb.code_row = code_row; lb.code_col = code_col;
+  const size_t smem = sizeof(AttnSmem) + sizeof(DecompSmem) + sizeof(float) * (kQTile * (dr.kh + dr.kw + 1) - 1);
+  static size_t smem_set = 0;
+  if (smem > smem_set) {
+    if (cudaFuncSetAttribute(attention_fwd_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                             static_cast<int>(smem)) != cudaSuccess)
+      return OPB_ERR_CUDA;
+    smem_set = smem;
+  }
+  const int q_chunks = (S + kQTile - 1) / kQTile;
+  const long grid = static_cast<long>(H) * q_chunks * B;
+  attention_fwd_kernel<true><<<static_cast<unsigned>(grid), 128, smem, stream>>>(
+      reinterpret_cast<const __nv_bfloat16*>(qkv), nullptr, nullptr, reinterpret_cast<__nv_bfloat16*>(out), lse, ln_stats,
+      B, S, H, 0, 0, lb, dr);
+  return cudaGetLastError() == cudaSuccess ? OPB_OK : OPB_ERR_CUDA;
 }
 
 // lut[h][l] = table[idx[l]][h]

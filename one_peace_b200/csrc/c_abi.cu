@@ -64,6 +64,25 @@ int opb_relpos_lut_build(const float* table, const int32_t* idx, float* lut, int
   return opb::relpos_lut_build(table, idx, lut, L, H, static_cast<cudaStream_t>(stream));
 }
 
+int opb_relpos_decomp_proj(const void* qkv, const float* rel_pos_h, const float* rel_pos_w, const int32_t* pos_y,
+                           const int32_t* pos_x, float q_unscale, float* rel_h, float* rel_w, int B, int S, int H, int kh,
+                           int kw, void* stream) {
+  if (!qkv || !rel_pos_h || !rel_pos_w || !pos_y || !pos_x || !rel_h || !rel_w) return OPB_ERR_INVALID;
+  return opb::relpos_decomp_proj(qkv, rel_pos_h, rel_pos_w, pos_y, pos_x, q_unscale, rel_h, rel_w, B, S, H, kh, kw,
+                                 static_cast<cudaStream_t>(stream));
+}
+
+int opb_attention_decomp_fwd(const void* qkv, const float* lut, int lut_len, const int32_t* code_row,
+                             const int32_t* code_col, const float* rel_h, const float* rel_w, const int32_t* key_y,
+                             const int32_t* key_x, int kh, int kw, void* out, float* lse, float* ln_stats, int B, int S,
+                             int H, void* stream) {
+  if (!qkv || !lut || !code_row || !code_col || !rel_h || !rel_w || !key_y || !key_x || !out) return OPB_ERR_INVALID;
+  opb::DecompRel dr;
+  dr.rel_h = rel_h; dr.rel_w = rel_w; dr.key_y = key_y; dr.key_x = key_x; dr.kh = kh; dr.kw = kw;
+  return opb::attention_decomp_fwd(qkv, lut, lut_len, code_row, code_col, dr, out, lse, ln_stats, B, S, H,
+                                   static_cast<cudaStream_t>(stream));
+}
+
 int opb_gemm_bf16_ex(const opb_gemm_args* a, void* stream) {
   if (a == nullptr || a->A == nullptr || a->B == nullptr || a->out == nullptr) return OPB_ERR_INVALID;
   if ((a->ln_mu == nullptr) != (a->ln_rstd == nullptr)) return OPB_ERR_INVALID;

@@ -27,6 +27,21 @@ constexpr int kAttnShortMaxLut = 4096;
 int attention_fwd_short(const void* qkv, const float* bias, const uint8_t* key_pad, void* out, float* lse, float* ln_stats,
                         int B, int S, int H, int s_pad, long bias_bstride, const LutBias& lb, cudaStream_t stream);
 int relpos_lut_build(const float* table, const int* idx, float* lut, int L, int H, cudaStream_t stream);
+// Decomposed relative-position terms of the detection backbone (csrc/relpos_decomp.cu, attention.cu): rel_h fp32
+// [B, H, S, kh], rel_w [B, H, S, kw]; key_y / key_x int32 [S] the key grid coordinates, kh * kw == S.
+struct DecompRel {
+  const float* rel_h = nullptr;
+  const float* rel_w = nullptr;
+  const int* key_y = nullptr;
+  const int* key_x = nullptr;
+  int kh = 0, kw = 0;
+};
+constexpr int kDecompMaxK = 256;     // grid side limit of both kernels (shared-memory staging of the tables and rows)
+int attention_decomp_fwd(const void* qkv, const float* lut, int lut_len, const int* code_row, const int* code_col,
+                         const DecompRel& dr, void* out, float* lse, float* ln_stats, int B, int S, int H,
+                         cudaStream_t stream);
+int relpos_decomp_proj(const void* qkv, const float* rel_pos_h, const float* rel_pos_w, const int* pos_y, const int* pos_x,
+                       float q_unscale, float* rel_h, float* rel_w, int B, int S, int H, int kh, int kw, cudaStream_t stream);
 int ln_stats_finalize(const float* partial, int parts, int rows, int dim, float eps, float* mu, float* rstd,
                       cudaStream_t stream);
 

@@ -132,6 +132,45 @@ def attention_tc(qkv, rp, key_pad, B, S, H, out=None, ln_stats=None, lse=None):
     return out
 
 
+def relpos_decomp_proj(qkv, rel_pos_h, rel_pos_w, pos_y, pos_x, B, S, H, kh, kw, q_unscale=8.0, rel_h=None, rel_w=None):
+    """Decomposed relative-position terms (include/onepeace_b200.h): -> (rel_h fp32 [B, H, S, kh], rel_w fp32 [B, H, S, kw]).
+    qkv bf16 [B*S, 3*H*64]; rel_pos_h / rel_pos_w fp32 [2k - 1, 64]; pos_y / pos_x int32 [S]."""
+    _need_cuda(qkv, rel_pos_h, rel_pos_w, pos_y, pos_x)
+    assert qkv.dtype == torch.bfloat16 and qkv.shape == (B * S, 3 * H * 64) and qkv.is_contiguous()
+    for t in (rel_pos_h, rel_pos_w):
+        assert t.dtype == torch.float32 and t.is_contiguous() and t.shape[1] == 64
+    assert rel_pos_h.shape[0] == 2 * kh - 1 and rel_pos_w.shape[0] == 2 * kw - 1
+    for t in (pos_y, pos_x):
+        assert t.dtype == torch.int32 and t.is_contiguous() and t.numel() == S
+    if rel_h is None:
+        rel_h = torch.empty(B, H, S, kh, dtype=torch.float32, device=qkv.device)
+    if rel_w is None:
+        rel_w = torch.empty(B, H, S, kw, dtype=torch.float32, device=qkv.device)
+    st = _lib.load().opb_relpos_decomp_proj(qkv.data_ptr(), rel_pos_h.data_ptr(), rel_pos_w.data_ptr(), pos_y.data_ptr(),
+                                            pos_x.data_ptr(), float(q_unscale), rel_h.data_ptr(), rel_w.data_ptr(), B, S, H,
+                                            kh, kw, _stream())
+    _lib.check(st, "opb_relpos_decomp_proj")
+    _count()
+    return rel_h, rel_w
+
+
+def attention_decomp(qkv, rp, rel_h, rel_w, key_y, key_x, B, S, H, kh, kw, out=None, ln_stats=None, lse=None):
+    """attention with the LUT-form bias `rp` (RelPosBias, no seg_split) plus rel_h[i][key_y[j]] + rel_w[i][key_x[j]]."""
+    D = H * 64
+    assert qkv.dtype == torch.bfloat16 and qkv.shape == (B * S, 3 * D) and qkv.is_contiguous()
+    assert int(getattr(rp, "seg_split", 0)) == 0
+    assert rel_h.shape == (B, H, S, kh) and rel_w.shape == (B, H, S, kw) and rel_h.is_contiguous() and rel_w.is_contiguous()
+    if out is None:
+        out = torch.empty(B * S, D, dtype=torch.bfloat16, device=qkv.device)
+    st = _lib.load().opb_attention_decomp_fwd(qkv.data_ptr(), rp.lut.data_ptr(), rp.lut.shape[1], rp.code_row.data_ptr(),
+                                              rp.code_col.data_ptr(), rel_h.data_ptr(), rel_w.data_ptr(), key_y.data_ptr(),
+                                              key_x.data_ptr(), kh, kw, out.data_ptr(), _ptr(lse), _ptr(ln_stats), B, S, H,
+                                              _stream())
+    _lib.check(st, "opb_attention_decomp_fwd")
+    _count()
+    return out
+
+
 def gemm_ln(a, w, epi, out, *, ln_mu=None, ln_rstd=None, ln_colsum=None, bias=None, colscale=None, gamma=None,
             resid=None, stats_out=None, out_bf16=None, cta_group=0, workspace=None, ln_partial=None, out_group=0,
             out_group_stride=0, out_row_offset=0, out_group_valid=0, resid_period=0, resid_row_offset=0):

@@ -76,3 +76,32 @@ class LutCache:
                                               # Q tile, up to 40 KB in a region of its own for long sequences)
             self._c[key] = None if r is None else tuple(torch.from_numpy(a).to(device) for a in r)
         return self._c[key]
+
+
+def grid_codes(side):
+    """Row-major side x side grid without a CLS row -> code = y * (2 side - 1) + x, so that code_i - code_j encodes (dy, dx)."""
+    p = np.arange(side * side, dtype=np.int64)
+    return (p // side) * (2 * side - 1) + p % side
+
+
+def grid_lut_index(side, order=None):
+    """LUT form of the bucket matrix ``make_image_bucket_position(side, ...)[1:, 1:]`` (the detection backbone's
+    ``rp_bucket`` / ``rp_bucket_window``): bucket[i][j] = code_i - code_j + maxc with maxc = (side - 1) * 2 side, so
+    lut_idx is the identity over the (2 side - 1)^2 table rows.  `order` (int64 [S'], row -> grid position) lays the codes
+    out in another row order, e.g. window-major.  Returns (lut_idx, code_row, code_col) int32 numpy, lengths padded to 4."""
+    c = grid_codes(side)
+    if order is not None:
+        c = c[np.asarray(order)]
+    maxc = (side - 1) * 2 * side
+    pad4 = lambda a: np.concatenate([a, np.zeros((-a.size) % 4, dtype=a.dtype)]).astype(np.int32)
+    return pad4(np.arange((2 * side - 1) ** 2, dtype=np.int64)), pad4(c + maxc), pad4(c)
+
+
+def window_major_order(side, window):
+    """Row order that keeps every window x window window of a row-major side x side grid contiguous, windows row-major
+    (detectron2's window_partition order).  Returns (perm int64 [side^2]: new row -> row-major position, y, x int64 [side^2]:
+    global grid coordinates of each new row, ly, lx: coordinates inside its window)."""
+    n = side // window
+    wy, wx, ly, lx = np.meshgrid(np.arange(n), np.arange(n), np.arange(window), np.arange(window), indexing="ij")
+    y, x = (wy * window + ly).reshape(-1), (wx * window + lx).reshape(-1)
+    return y * side + x, y, x, ly.reshape(-1), lx.reshape(-1)
