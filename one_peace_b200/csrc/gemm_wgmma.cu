@@ -2,15 +2,17 @@
 //
 //   * operands are bf16, K-major (activations [rows, K], nn.Linear weights [out, in]) or MN-major (given as [K, rows]: the
 //     weight gradient dW = dY^T X and the InfoNCE gradient), staged into shared memory by TMA with the 128-byte swizzle,
-//     BLOCK_K = 64, four pipeline stages (4 x 48 KB);
+//     BLOCK_K = 64, four pipeline stages (4 x 48 KB; three in the kernels that stage their output tile, see below);
 //   * persistent: one CTA per SM walks 128 x 256 output tiles (grouped in bands of row panels, see kBandM) with the stage ring
 //     running on across tiles, so the next tile's loads overlap the current tile's epilogue.  Three warpgroups: in warpgroup 0
 //     one thread issues the TMA loads and warps 1-3 stage the next tile's epilogue operands (LayerNorm row statistics, column
 //     vectors) in shared memory (register budget lowered with setmaxnreg); warpgroups 1 and 2 own 64 rows each and issue
 //     wgmma.m64n256k16 (fp32 accumulators in registers, 128 per thread);
-//   * the fused epilogue runs on the accumulator fragments and stores straight to global memory.  A thread holds two rows
-//     (r, r + 8) x 2 adjacent columns of every 8-column group, so per-row reductions (LayerNorm statistics, soft-max partials)
-//     are finished with two shuffles inside a quad.
+//   * the fused epilogue runs on the accumulator fragments.  A thread holds two rows (r, r + 8) x 2 adjacent columns of every
+//     8-column group, so per-row reductions (LayerNorm statistics, soft-max partials) are finished with two shuffles inside a
+//     quad.  gemm_bf16_kernel stores the results straight to global memory.  gemm_bf16_tma_out_kernel (the bf16 epilogues on
+//     a plain row-major output) writes them with stmatrix into a per-warpgroup shared-memory copy of its 64 output rows and
+//     one thread hands that to TMA bulk stores, so the stores drain while the warpgroup runs the next tile's mainloop.
 //
 // Fused epilogues (what the reference runs as separate ATen kernels, SURVEY.md 2.5 K1'/K3/K4):
 //   EPI_STORE_BF16 : out_bf16 = (acc + bias[n]) * colscale[n]        (q/k/v projection, q pre-scaled;
@@ -31,7 +33,8 @@ namespace opb {
 constexpr int kBlockM = 128;   // rows of A per CTA (two consumer warpgroups x 64)
 constexpr int kBlockN = 256;   // output columns per tile = wgmma N
 constexpr int kBlockK = 64;    // 64 bf16 = 128 bytes = one swizzle row
-constexpr int kStages = 4;
+constexpr int kStages = 4;          // gemm_bf16_kernel
+constexpr int kStagesTmaOut = 3;    // gemm_bf16_tma_out_kernel: the output staging area takes the fourth stage's room
 constexpr int kABytes = kBlockM * kBlockK * 2;   // 16 KB
 constexpr int kBBytes = kBlockN * kBlockK * 2;   // 32 KB
 constexpr int kStageBytes = kABytes + kBBytes;
@@ -51,7 +54,17 @@ struct EpiOperands {
   float colsum[kBlockN], bias[kBlockN], gamma[kBlockN], colscale[kBlockN];   // the tile's slices of the column vectors
 };
 constexpr int kStagerThreads = 96;   // warps 1-3 of warpgroup 0
-constexpr int kSmemBytes = kStages * kStageBytes + 1024 + 2 * sizeof(EpiOperands) + 1024;   // + barriers + alignment slack
+// Output staging of gemm_bf16_tma_out_kernel, right after the stage ring: per consumer warpgroup its 64 rows x 256 bf16
+// columns as four 64 x 64 boxes (8 KB, 128-byte swizzle), the box layout of the output tensor map.
+constexpr int kOutBoxBytes = 64 * 128;
+constexpr int kOutStageBytes = 4 * kOutBoxBytes;
+// stage ring (+ output staging) + barriers + epilogue operands + alignment slack
+constexpr int smem_bytes(int stages, bool tma_out) {
+  return stages * kStageBytes + (tma_out ? 2 * kOutStageBytes : 0) + 1024 + 2 * sizeof(EpiOperands) + 1024;
+}
+constexpr int kSmemBytes = smem_bytes(kStages, false);
+constexpr int kSmemBytesTmaOut = smem_bytes(kStagesTmaOut, true);
+static_assert(kSmemBytesTmaOut <= 227 * 1024, "output staging does not fit next to the stage ring");
 
 struct GemmGeom {
   int M, N, K;          // per group: rows, output columns, reduction length (= taps * kb_inner * 64 when windowed)
@@ -155,7 +168,7 @@ OPB_DEVICE float quad_sum(float v) {
 
 // One tile's k-blocks.  `it0` counts the k-blocks this CTA consumed for earlier tiles: the stage ring and its phases run on
 // across tiles, so the producer fills the next tile's stages while the current tile's epilogue runs.
-template <int TA, int TB>
+template <int TA, int TB, int S>
 OPB_DEVICE void mainloop(float (&d)[128], uint8_t* smem, uint64_t* full, uint64_t* empty, int num_k_blocks, int cw,
                          uint32_t it0) {
   // descriptor advance per 16-deep wgmma: 32 B inside the swizzle row (K-major) or two 8-row k groups = 2048 B (MN-major)
@@ -163,8 +176,8 @@ OPB_DEVICE void mainloop(float (&d)[128], uint8_t* smem, uint64_t* full, uint64_
   const bool signal = (threadIdx.x & 31) == 0;
   for (int kb = 0; kb < num_k_blocks; ++kb) {
     const uint32_t it = it0 + kb;
-    const uint32_t s = it % kStages;
-    mbar_wait_quiet(&full[s], (it / kStages) & 1);
+    const uint32_t s = it % S;
+    mbar_wait_quiet(&full[s], (it / S) & 1);
     const uint32_t sa = smem_u32(smem + s * kStageBytes) + cw * 8192;   // this warpgroup's 64 rows (K-major) / M chunk (MN-major)
     const uint32_t sb = smem_u32(smem + s * kStageBytes + kABytes);
     fence_acc(d);
@@ -179,13 +192,59 @@ OPB_DEVICE void mainloop(float (&d)[128], uint8_t* smem, uint64_t* full, uint64_
       wgmma_wait<1>();
       fence_acc(d);
       __syncwarp();
-      if (signal) mbar_arrive(&empty[(it - 1) % kStages]);
+      if (signal) mbar_arrive(&empty[(it - 1) % S]);
     }
   }
   wgmma_wait<0>();
   fence_acc(d);
   __syncwarp();
-  if (signal) mbar_arrive(&empty[(it0 + num_k_blocks - 1) % kStages]);
+  if (signal) mbar_arrive(&empty[(it0 + num_k_blocks - 1) % S]);
+}
+
+// Output staging (gemm_bf16_tma_out_kernel).  The bf16 pairs v[0 .. kGroups) of fragment row h, one per 8-column group, go
+// into the warpgroup's staging area with one stmatrix.x4 per 4 groups: matrix i is the 8 x 8 block of rows (warp, h) and
+// column group 4 q + i, lane l gives the address of row l & 7 of matrix l >> 3.  With the 128-byte swizzle the 8 rows of a
+// matrix hit 8 different 16-byte bank groups, so the stores are conflict-free.  Called after the loop that computes v: an
+// aligned (convergent) instruction inside it would keep the compiler from specialising that loop on the epilogue's flags.
+template <int kGroups>
+OPB_DEVICE void stage_out_row(uint32_t stage, int h, const uint32_t (&v)[kGroups]) {
+  const int lane = threadIdx.x & 31;
+  const int row = ((threadIdx.x & 127) >> 5) * 16 + 8 * h + (lane & 7);
+#pragma unroll
+  for (int q = 0; q < kGroups / 4; ++q) {
+    const int cg = 4 * q + (lane >> 3);
+    const uint32_t addr = stage + (cg >> 3) * kOutBoxBytes + sw128_off(row, cg & 7);
+    asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(v[4 * q]),
+                 "r"(v[4 * q + 1]), "r"(v[4 * q + 2]), "r"(v[4 * q + 3]));
+  }
+}
+
+OPB_DEVICE void warpgroup_bar_sync(int cw) {
+  if (cw == 0) asm volatile("bar.sync 1, 128;" ::: "memory");
+  else asm volatile("bar.sync 2, 128;" ::: "memory");
+}
+
+// Before the staging area is written again: the previous tile's bulk stores have finished reading it.  Only the thread that
+// issued them can wait for them; the named barrier (one per consumer warpgroup, id 1 + cw) passes that on to its warps.
+OPB_DEVICE void acquire_out_stage(int cw) {
+  if ((threadIdx.x & 127) == 0) bulk_wait_read<0>();
+  warpgroup_bar_sync(cw);
+}
+
+// After the epilogue has staged the tile: make the shared-memory writes visible to the async proxy, meet at the warpgroup's
+// barrier, and let one thread store the boxes of rows row0 .. row0 + 63 that hold output, as one bulk group.  Rows >= rows
+// and columns >= cols of a box are clipped by the tensor map; boxes wholly outside are not issued.
+OPB_DEVICE void store_out_tile(const CUtensorMap& tm_out, uint8_t* stage, int row0, int col0, int rows, int cols, int boxes,
+                               int cw) {
+  fence_proxy_async();
+  warpgroup_bar_sync(cw);
+  if ((threadIdx.x & 127) == 0) {
+    if (row0 < rows) {
+      for (int b = 0; b < boxes; ++b)
+        if (col0 + 64 * b < cols) tma_store_2d(&tm_out, stage + b * kOutBoxBytes, col0 + 64 * b, row0);
+    }
+    bulk_commit();
+  }
 }
 
 // the epilogues that take their operands from EpiOperands (the contrastive-head ones read none of them)
@@ -213,9 +272,11 @@ OPB_DEVICE void stage_epi_operands(EpiOperands* st, const GemmEpilogue& ep, cons
   }
 }
 
-template <int EPI>
-OPB_DEVICE void epilogue(const float (&d)[128], const GemmEpilogue& ep, const GemmGeom& geo, const EpiOperands* st, int m_blk,
-                         int n_blk, int grp, int cw) {
+// kTmaOut: the bf16 results go to the warpgroup's output staging area at shared address `out_stage` (all 64 rows and every
+// column of the tile; store_out_tile clips them) instead of global memory.  The values and their order are the same.
+template <int EPI, bool kTmaOut>
+OPB_DEVICE void epilogue(const float (&d)[128], const GemmEpilogue& ep, const GemmGeom& geo, const EpiOperands* st,
+                         uint32_t out_stage, int m_blk, int n_blk, int grp, int cw) {
   const int M = geo.M, N = geo.N;
   const int t = threadIdx.x & 127;
   const int lane = t & 31;
@@ -314,6 +375,7 @@ OPB_DEVICE void epilogue(const float (&d)[128], const GemmEpilogue& ep, const Ge
       float st_sum = 0.f, st_sq = 0.f;   // partial statistics of the stored values (next LayerNorm)
       if constexpr (EPI == EPI_GEGLU_BF16) {
         __nv_bfloat16* out = reinterpret_cast<__nv_bfloat16*>(ep.out) + out_row * ep.ldo + n_blk * (kBlockN / 2);
+        uint32_t packed[16];
 #pragma unroll
         for (int j = 0; j < 16; ++j) {
           const int tc = 8 * j + 2 * quad;    // gate column inside the tile; its linear partner is tc + 128
@@ -331,8 +393,10 @@ OPB_DEVICE void epilogue(const float (&d)[128], const GemmEpilogue& ep, const Ge
           const float u0 = gelu_erf(g0) * l0, u1 = gelu_erf(g1) * l1;
           st_sum += u0 + u1;
           st_sq += u0 * u0 + u1 * u1;
-          if (row_ok) *reinterpret_cast<uint32_t*>(out + tc) = pack_bf16x2(u0, u1);
+          if constexpr (kTmaOut) packed[j] = pack_bf16x2(u0, u1);
+          else if (row_ok) *reinterpret_cast<uint32_t*>(out + tc) = pack_bf16x2(u0, u1);
         }
+        if constexpr (kTmaOut) stage_out_row(out_stage, h, packed);
         st_sum = quad_sum(st_sum);
         st_sq = quad_sum(st_sq);
         if (row_ok && quad == 0 && ep.stats_out != nullptr) {   // [2 * n_tiles, M] records, the second of a tile is zero
@@ -345,6 +409,7 @@ OPB_DEVICE void epilogue(const float (&d)[128], const GemmEpilogue& ep, const Ge
         // place), so the compiler cannot hoist a load above an earlier store: loaded inside the column loop, every column
         // group would wait for its own global round trip.  Loading ahead is safe because an element of `resid` that is also
         // an output element is the one this thread writes from the same fragment slot (gemm_bf16 refuses any other overlap).
+        uint32_t packed[32];
 #pragma unroll
         for (int jb = 0; jb < 32; jb += kResidBatch) {
           float2 res[kResidBatch];
@@ -363,7 +428,7 @@ OPB_DEVICE void epilogue(const float (&d)[128], const GemmEpilogue& ep, const Ge
             const int j = jb + jj;
             const int lc = 8 * j + 2 * quad;           // column inside the tile
             const int tc = col0 + lc;                  // column inside the group
-            if (tc >= N) continue;
+            if (!kTmaOut && tc >= N) continue;         // (staged: columns >= N hold zeros and are clipped)
             const int col = gcol0 + tc;
             float x0 = d[4 * j + 2 * h], x1 = d[4 * j + 2 * h + 1];
             if (has_ln) {
@@ -380,7 +445,11 @@ OPB_DEVICE void epilogue(const float (&d)[128], const GemmEpilogue& ep, const Ge
                 x0 *= s.x; x1 *= s.y;
               }
               if constexpr (EPI == EPI_GELU_BF16) { x0 = gelu_erf(x0); x1 = gelu_erf(x1); }
-              if (row_ok) *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(ep.out) + out_row * ep.ldo + col) = pack_bf16x2(x0, x1);
+              if constexpr (kTmaOut) {
+                packed[j] = pack_bf16x2(x0, x1);
+              } else {
+                if (row_ok) *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(ep.out) + out_row * ep.ldo + col) = pack_bf16x2(x0, x1);
+              }
             } else {
               if constexpr (EPI == EPI_RESID_F32) {
                 if (ep.gamma != nullptr) {
@@ -399,6 +468,7 @@ OPB_DEVICE void epilogue(const float (&d)[128], const GemmEpilogue& ep, const Ge
             }
           }
         }
+        if constexpr (kTmaOut) stage_out_row(out_stage, h, packed);
         if constexpr (EPI == EPI_RESID_F32) {
           st_sum = quad_sum(st_sum);
           st_sq = quad_sum(st_sq);
@@ -432,20 +502,22 @@ OPB_DEVICE TileCoord tile_coord(int unit, int num_m_tiles, int num_n_tiles, int 
 }
 
 // Persistent: the grid holds as many CTAs as can be resident and CTA b runs units b, b + gridDim.x, ...  Barrier set-up and
-// descriptor prefetch happen once per CTA.
-template <int EPI>
-__global__ void __launch_bounds__(kThreads, 1)
-gemm_bf16_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__ CUtensorMap tm_b, const GemmEpilogue ep,
-                 const GemmGeom geo) {
+// descriptor prefetch happen once per CTA.  The body of both kernels: S pipeline stages; kTmaOut stages the bf16 output tile
+// in shared memory and stores it with TMA through tm_out (not used otherwise).
+template <int EPI, int S, bool kTmaOut>
+OPB_DEVICE void gemm_body(const CUtensorMap& tm_a, const CUtensorMap& tm_b, const CUtensorMap* tm_out, const GemmEpilogue& ep,
+                          const GemmGeom& geo) {
   // no static shared memory: the dynamic window starts at the 1024-aligned base the 128-byte swizzle needs (checked)
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = smem_raw;
   if ((smem_u32(smem) & 1023u) != 0) __trap();
-  uint64_t* full = reinterpret_cast<uint64_t*>(smem + kStages * kStageBytes);
-  uint64_t* empty = full + kStages;
-  uint64_t* epi_full = empty + kStages;   // [2] operands of the buffer's tile are staged
+  uint8_t* out_stage = smem + S * kStageBytes;   // [2 consumer warpgroups][kOutStageBytes] (kTmaOut)
+  uint8_t* bars = out_stage + (kTmaOut ? 2 * kOutStageBytes : 0);
+  uint64_t* full = reinterpret_cast<uint64_t*>(bars);
+  uint64_t* empty = full + S;
+  uint64_t* epi_full = empty + S;         // [2] operands of the buffer's tile are staged
   uint64_t* epi_empty = epi_full + 2;     // [2] the buffer's epilogue is done reading
-  EpiOperands* epi_ops = reinterpret_cast<EpiOperands*>(smem + kStages * kStageBytes + 1024);
+  EpiOperands* epi_ops = reinterpret_cast<EpiOperands*>(bars + 1024);
 
   const int wg = threadIdx.x >> 7;
   const int num_m_tiles = (geo.M + kBlockM - 1) / kBlockM;
@@ -453,12 +525,13 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant
   const int pieces = geo.kb_per_piece > 0 ? (geo.num_k_blocks + geo.kb_per_piece - 1) / geo.kb_per_piece : 1;
   const int units = num_m_tiles * num_n_tiles * geo.groups * pieces;
   // split-K pieces store raw accumulators and need no epilogue operands
-  const bool staged = epi_staged(EPI) && geo.kb_per_piece == 0;
+  const bool staged = epi_staged(EPI) && (kTmaOut || geo.kb_per_piece == 0);
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tm_a);
     tma_prefetch_desc(&tm_b);
-    for (int i = 0; i < kStages; ++i) {
+    if constexpr (kTmaOut) tma_prefetch_desc(tm_out);
+    for (int i = 0; i < S; ++i) {
       mbar_init(&full[i], 1);
       mbar_init(&empty[i], 8);   // lane 0 of each of the 8 consumer warps
     }
@@ -474,7 +547,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant
     asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
     if (threadIdx.x == 0) {
       // ===================== TMA producer =====================
-      uint32_t it = 0;   // k-blocks issued by this CTA: stage it % kStages, phase (it / kStages) & 1
+      uint32_t it = 0;   // k-blocks issued by this CTA: stage it % S, phase (it / S) & 1
       for (int unit = blockIdx.x; unit < units; unit += gridDim.x) {
         const TileCoord tc = tile_coord(unit, num_m_tiles, num_n_tiles, geo.groups);
         const int kb0 = geo.kb_per_piece > 0 ? tc.piece * geo.kb_per_piece : 0;
@@ -484,8 +557,8 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant
         const int a_c0 = tc.grp * geo.a_group_c0;
         int kin = kb0 % geo.kb_inner, tap = kb0 / geo.kb_inner;
         for (int kb = kb0; kb < kb1; ++kb, ++it) {
-          const uint32_t s = it % kStages;
-          mbar_wait_quiet(&empty[s], ((it / kStages) & 1) ^ 1);
+          const uint32_t s = it % S;
+          mbar_wait_quiet(&empty[s], ((it / S) & 1) ^ 1);
           uint8_t* sa = smem + s * kStageBytes;
           uint8_t* sb = sa + kABytes;
           mbar_arrive_expect_tx(&full[s], kStageBytes);     // out-of-bounds box elements are zero-filled and counted
@@ -518,6 +591,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant
     // ===================== consumers: wgmma + epilogue =====================
     asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
     const int cw = wg - 1;
+    uint8_t* my_stage = out_stage + cw * kOutStageBytes;
     float d[128];
 #pragma unroll
     for (int i = 0; i < 128; ++i) d[i] = 0.f;
@@ -527,14 +601,14 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant
       const int kb0 = geo.kb_per_piece > 0 ? tc.piece * geo.kb_per_piece : 0;
       const int kb1 = geo.kb_per_piece > 0 ? min(geo.num_k_blocks, kb0 + geo.kb_per_piece) : geo.num_k_blocks;
       if (geo.a_mn) {
-        if (geo.b_mn) mainloop<1, 1>(d, smem, full, empty, kb1 - kb0, cw, it);
-        else mainloop<1, 0>(d, smem, full, empty, kb1 - kb0, cw, it);
+        if (geo.b_mn) mainloop<1, 1, S>(d, smem, full, empty, kb1 - kb0, cw, it);
+        else mainloop<1, 0, S>(d, smem, full, empty, kb1 - kb0, cw, it);
       } else {
-        if (geo.b_mn) mainloop<0, 1>(d, smem, full, empty, kb1 - kb0, cw, it);
-        else mainloop<0, 0>(d, smem, full, empty, kb1 - kb0, cw, it);
+        if (geo.b_mn) mainloop<0, 1, S>(d, smem, full, empty, kb1 - kb0, cw, it);
+        else mainloop<0, 0, S>(d, smem, full, empty, kb1 - kb0, cw, it);
       }
       it += kb1 - kb0;
-      if (geo.kb_per_piece > 0) {
+      if (!kTmaOut && geo.kb_per_piece > 0) {   // (the staged-output kernel never runs split-K)
         // split-K piece: raw partial accumulators of all m_pad rows into this piece's slab (plain stores, no atomics)
         const int t = threadIdx.x & 127, lane = t & 31;
         const int r0 = tc.m_blk * kBlockM + cw * 64 + (t >> 5) * 16 + (lane >> 2);
@@ -550,14 +624,43 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant
         }
       } else if (staged) {
         mbar_wait_quiet(&epi_full[j & 1], (j >> 1) & 1);
-        epilogue<EPI>(d, ep, geo, &epi_ops[j & 1], tc.m_blk, tc.n_blk, tc.grp, cw);
+        if constexpr (kTmaOut) acquire_out_stage(cw);
+        epilogue<EPI, kTmaOut>(d, ep, geo, &epi_ops[j & 1], smem_u32(my_stage), tc.m_blk, tc.n_blk, tc.grp, cw);
         __syncwarp();
         if ((threadIdx.x & 31) == 0) mbar_arrive(&epi_empty[j & 1]);
+        if constexpr (kTmaOut) {
+          // GeGLU writes kBlockN / 2 columns per tile: two boxes
+          constexpr int cols_per_tile = EPI == EPI_GEGLU_BF16 ? kBlockN / 2 : kBlockN;
+          store_out_tile(*tm_out, my_stage, tc.m_blk * kBlockM + cw * 64, tc.n_blk * cols_per_tile, geo.M,
+                         EPI == EPI_GEGLU_BF16 ? geo.N / 2 : geo.N, cols_per_tile / 64, cw);
+        }
       } else {
-        epilogue<EPI>(d, ep, geo, nullptr, tc.m_blk, tc.n_blk, tc.grp, cw);
+        epilogue<EPI, false>(d, ep, geo, nullptr, 0, tc.m_blk, tc.n_blk, tc.grp, cw);
       }
     }
+    // the staging area must outlive the last bulk stores
+    if constexpr (kTmaOut) {
+      if ((threadIdx.x & 127) == 0) bulk_wait_all<0>();
+    }
   }
+}
+
+template <int EPI>
+__global__ void __launch_bounds__(kThreads, 1)
+gemm_bf16_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__ CUtensorMap tm_b, const GemmEpilogue ep,
+                 const GemmGeom geo) {
+  gemm_body<EPI, kStages, false>(tm_a, tm_b, nullptr, ep, geo);
+}
+
+// The bf16 epilogues with the output tile staged in shared memory and stored by TMA through tm_out (rows M, columns N, or
+// N / 2 for GeGLU; box 64 x 64, 128-byte swizzle).  Taken only for a single group, no split-K and no row remapping (see
+// tma_out_applies).
+template <int EPI>
+__global__ void __launch_bounds__(kThreads, 1)
+gemm_bf16_tma_out_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__ CUtensorMap tm_b,
+                         const __grid_constant__ CUtensorMap tm_out, const GemmEpilogue ep, const GemmGeom geo) {
+  static_assert(EPI == EPI_STORE_BF16 || EPI == EPI_GELU_BF16 || EPI == EPI_GEGLU_BF16, "bf16 epilogues only");
+  gemm_body<EPI, kStagesTmaOut, true>(tm_a, tm_b, &tm_out, ep, geo);
 }
 
 // Epilogue of the small-M split-K schedule: x = sum of the piece slabs (fixed order), then the EPI_RESID_F32 epilogue
@@ -692,38 +795,61 @@ int make_tmap_bf16_batched(CUtensorMap* out, const void* ptr, uint64_t cols, uin
   return r == CUDA_SUCCESS ? OPB_OK : OPB_ERR_CUDA;
 }
 
-template <int EPI>
-static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, const GemmEpilogue& ep, const GemmGeom& geo,
-                       cudaStream_t stream) {
-  auto kern = gemm_bf16_kernel<EPI>;
+// kTmaOut: gemm_bf16_tma_out_kernel<EPI> with the output tensor map `to`; otherwise gemm_bf16_kernel<EPI> (`to` unused)
+template <int EPI, bool kTmaOut>
+static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap* to, const GemmEpilogue& ep,
+                       const GemmGeom& geo, cudaStream_t stream) {
+  constexpr int smem = kTmaOut ? kSmemBytesTmaOut : kSmemBytes;
+  const void* kern;
+  if constexpr (kTmaOut) kern = reinterpret_cast<const void*>(gemm_bf16_tma_out_kernel<EPI>);
+  else kern = reinterpret_cast<const void*>(gemm_bf16_kernel<EPI>);
   static int resident = 0;   // CTAs resident at once over the whole GPU
   if (resident == 0) {
-    if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes) != cudaSuccess)
+    if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) != cudaSuccess)
       return OPB_ERR_CUDA;
     int per_sm = 0;
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, kThreads, kSmemBytes) != cudaSuccess || per_sm < 1)
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, kThreads, smem) != cudaSuccess || per_sm < 1)
       return OPB_ERR_CUDA;
     resident = per_sm * sm_count();
   }
   const int pieces = geo.kb_per_piece > 0 ? (geo.num_k_blocks + geo.kb_per_piece - 1) / geo.kb_per_piece : 1;
   const long units = static_cast<long>((geo.M + kBlockM - 1) / kBlockM) * ((geo.N + kBlockN - 1) / kBlockN) * geo.groups * pieces;
   const unsigned grid = static_cast<unsigned>(units < resident ? units : resident);
-  kern<<<grid, kThreads, kSmemBytes, stream>>>(ta, tb, ep, geo);
+  if constexpr (kTmaOut) gemm_bf16_tma_out_kernel<EPI><<<grid, kThreads, smem, stream>>>(ta, tb, *to, ep, geo);
+  else gemm_bf16_kernel<EPI><<<grid, kThreads, smem, stream>>>(ta, tb, ep, geo);
   return cudaGetLastError() == cudaSuccess ? OPB_OK : OPB_ERR_CUDA;
 }
 
-static int dispatch_gemm(int epi, const CUtensorMap& ta, const CUtensorMap& tb, const GemmEpilogue& ep, const GemmGeom& geo,
-                         cudaStream_t stream) {
+// `to` != nullptr: the output tensor map of the TMA-store kernel (bf16 epilogues only, see tma_out_applies)
+static int dispatch_gemm(int epi, const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap* to, const GemmEpilogue& ep,
+                         const GemmGeom& geo, cudaStream_t stream) {
+  if (to != nullptr) {
+    switch (epi) {
+      case EPI_STORE_BF16: return launch_gemm<EPI_STORE_BF16, true>(ta, tb, to, ep, geo, stream);
+      case EPI_GELU_BF16: return launch_gemm<EPI_GELU_BF16, true>(ta, tb, to, ep, geo, stream);
+      case EPI_GEGLU_BF16: return launch_gemm<EPI_GEGLU_BF16, true>(ta, tb, to, ep, geo, stream);
+      default: return OPB_ERR_INVALID;
+    }
+  }
   switch (epi) {
-    case EPI_STORE_BF16: return launch_gemm<EPI_STORE_BF16>(ta, tb, ep, geo, stream);
-    case EPI_GELU_BF16: return launch_gemm<EPI_GELU_BF16>(ta, tb, ep, geo, stream);
-    case EPI_GEGLU_BF16: return launch_gemm<EPI_GEGLU_BF16>(ta, tb, ep, geo, stream);
-    case EPI_RESID_F32: return launch_gemm<EPI_RESID_F32>(ta, tb, ep, geo, stream);
-    case EPI_STORE_F32: return launch_gemm<EPI_STORE_F32>(ta, tb, ep, geo, stream);
-    case EPI_LSE_PARTIAL: return launch_gemm<EPI_LSE_PARTIAL>(ta, tb, ep, geo, stream);
-    case EPI_SOFTMAX_GRAD: return launch_gemm<EPI_SOFTMAX_GRAD>(ta, tb, ep, geo, stream);
+    case EPI_STORE_BF16: return launch_gemm<EPI_STORE_BF16, false>(ta, tb, nullptr, ep, geo, stream);
+    case EPI_GELU_BF16: return launch_gemm<EPI_GELU_BF16, false>(ta, tb, nullptr, ep, geo, stream);
+    case EPI_GEGLU_BF16: return launch_gemm<EPI_GEGLU_BF16, false>(ta, tb, nullptr, ep, geo, stream);
+    case EPI_RESID_F32: return launch_gemm<EPI_RESID_F32, false>(ta, tb, nullptr, ep, geo, stream);
+    case EPI_STORE_F32: return launch_gemm<EPI_STORE_F32, false>(ta, tb, nullptr, ep, geo, stream);
+    case EPI_LSE_PARTIAL: return launch_gemm<EPI_LSE_PARTIAL, false>(ta, tb, nullptr, ep, geo, stream);
+    case EPI_SOFTMAX_GRAD: return launch_gemm<EPI_SOFTMAX_GRAD, false>(ta, tb, nullptr, ep, geo, stream);
     default: return OPB_ERR_INVALID;
   }
+}
+
+// The bf16 epilogues store through shared memory and TMA (gemm_bf16_tma_out_kernel) when the output is one plain row-major
+// bf16 matrix a tensor map can describe: no split-K (its pieces store fp32 slabs), one group (the 256 columns of a grouped-
+// window tile would run into the next group's columns), no row remapping, a 16-byte aligned base and row pitch, and a pitch no
+// smaller than the row.  Every other call keeps the direct-store kernel.
+static bool tma_out_applies(int epi, const GemmEpilogue& ep, const GemmGeom& geo, long out_cols) {
+  return (epi == EPI_STORE_BF16 || epi == EPI_GELU_BF16 || epi == EPI_GEGLU_BF16) && geo.kb_per_piece == 0 && geo.groups == 1 &&
+         ep.out_group == 0 && (reinterpret_cast<uintptr_t>(ep.out) & 15) == 0 && (ep.ldo * 2) % 16 == 0 && ep.ldo >= out_cols;
 }
 
 // Bytes [begin, end) spanned by rows lo..hi of a row-major matrix with pitch ld and `cols` columns of `esz` bytes.
@@ -813,7 +939,11 @@ int gemm_bf16(const void* A, int lda, const void* B, int ldb, int M, int N, int 
   if (rc != OPB_OK) return rc;
   rc = make_tmap_bf16_2d(&tb, B, N, K, ldb, kBlockN);
   if (rc != OPB_OK) return rc;
-  rc = dispatch_gemm(epi, ta, tb, ep, geo, stream);
+  const long out_cols = epi == EPI_GEGLU_BF16 ? N / 2 : N;
+  CUtensorMap to;
+  const bool tma_out = tma_out_applies(epi, ep, geo, out_cols);
+  if (tma_out && (rc = make_tmap_bf16_2d(&to, ep.out, M, out_cols, ep.ldo, 64)) != OPB_OK) return rc;
+  rc = dispatch_gemm(epi, ta, tb, tma_out ? &to : nullptr, ep, geo, stream);
   if (rc != OPB_OK || geo.kb_per_piece == 0) return rc;
   gemm_split_epilogue_kernel<<<dim3(M, n_tiles), 256, 0, stream>>>(ep, geo, pieces, epi);
   return cudaGetLastError() == cudaSuccess ? OPB_OK : OPB_ERR_CUDA;
@@ -835,7 +965,10 @@ int gemm_bf16_t(const void* A, int lda, int a_mn, const void* B, int ldb, int b_
   if (rc != OPB_OK) return rc;
   rc = b_mn ? make_tmap_bf16_2d(&tb, B, K, N, ldb, 64) : make_tmap_bf16_2d(&tb, B, N, K, ldb, kBlockN);
   if (rc != OPB_OK) return rc;
-  return dispatch_gemm(epi, ta, tb, ep, geo, stream);
+  CUtensorMap to;
+  const bool tma_out = tma_out_applies(epi, ep, geo, N);
+  if (tma_out && (rc = make_tmap_bf16_2d(&to, ep.out, M, N, ep.ldo, 64)) != OPB_OK) return rc;
+  return dispatch_gemm(epi, ta, tb, tma_out ? &to : nullptr, ep, geo, stream);
 }
 
 int gemm_bf16_grouped_window(const void* X, const void* W, int rows, int groups, int c_pad, int taps, int n_per_group,
@@ -857,7 +990,7 @@ int gemm_bf16_grouped_window(const void* X, const void* W, int rows, int groups,
   if (rc != OPB_OK) return rc;
   rc = make_tmap_bf16_2d(&tb, W, static_cast<uint64_t>(groups) * n_per_group, geo.K, geo.K, kBlockN);
   if (rc != OPB_OK) return rc;
-  return dispatch_gemm(epi, ta, tb, ep, geo, stream);
+  return dispatch_gemm(epi, ta, tb, nullptr, ep, geo, stream);
 }
 
 }  // namespace opb
