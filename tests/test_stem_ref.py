@@ -5,7 +5,9 @@ emulation of their kernels.
 activations and gradients, fp32 records), with the row maps of the C header (pixel merges, the CLS-row shift, window
 gathers, strided rows).  The Functions run unchanged on it, packs, views and shifts included, from a fresh copy of the
 autograd module's source.  Their results must stay within the bounds, and each planted mistake (a one-line change of that
-source, or of one emulated kernel) must exceed them at least 100-fold somewhere."""
+source, or of one emulated kernel) must exceed them at least 100-fold somewhere.  tests/test_head_ref.py runs the
+classification heads, the criteria and the pretraining-path Functions on the same ``Emu``, ``Recorder`` and
+``functions``."""
 import inspect
 from types import SimpleNamespace
 
@@ -15,22 +17,27 @@ import torch.nn.functional as F
 
 import kernel_ref as R
 import stem_ref as SR
+import test_classify_host_logic as CH
+from grounding_ref import refcoco
 from one_peace_b200 import autograd as AG
+from vit_ref import head_bwd, head_fwd
 
 BF = torch.bfloat16
 MISS = 100.0            # a planted mistake must use at least this many times its bound
 
 
 class Emu:
-    """fp64 emulation of the kernels the stems and the head call (``one_peace_b200.kernels`` signatures).  Flags plant
-    mistakes inside a kernel: ``text_pad_grad`` (padding tokens get a gradient), ``text_pos_shift`` (position gradients
-    one row early), ``l2_no_radial`` (l2-normalize backward without the radial projection)."""
+    """fp64 emulation of the kernels the training Functions around the encoder stack call (``one_peace_b200.kernels``
+    signatures).  Flags plant mistakes inside a kernel: ``text_pad_grad`` (padding tokens get a gradient),
+    ``text_pos_shift`` (position gradients one row early), ``l2_no_radial`` (l2-normalize backward without the radial
+    projection), ``scatter_overwrite`` (row_scatter_add stores instead of adding, so a repeated index keeps one row)."""
     EPI_STORE_BF16, EPI_GEGLU_BF16, EPI_RESID_F32, EPI_STORE_F32, EPI_GELU_BF16 = 0, 1, 2, 3, 4
 
     def __init__(self, **flags):
         self.text_pad_grad = flags.pop("text_pad_grad", False)
         self.text_pos_shift = flags.pop("text_pos_shift", False)
         self.l2_no_radial = flags.pop("l2_no_radial", False)
+        self.scatter_overwrite = flags.pop("scatter_overwrite", False)
         assert not flags
 
     @staticmethod
@@ -136,13 +143,13 @@ class Emu:
 
     def l2_normalize_rows(self, x):
         X = x.double()
-        return (X / X.norm(dim=1, keepdim=True)).float()
+        return (X / X.norm(dim=1, keepdim=True).clamp_min(1e-12)).float()
 
-    def l2_normalize_bwd(self, x, dy):
+    def l2_normalize_bwd(self, x, dy, want_f32=False):
         X, G = x.double(), dy.double()
         n = X.norm(dim=1, keepdim=True)
         dx = G / n if self.l2_no_radial else G / n - X * (X * G).sum(1, keepdim=True) / n ** 3
-        return dx.to(BF)
+        return (dx.to(BF), dx.float()) if want_f32 else dx.to(BF)
 
     def text_embed(self, tokens, table, pos, cls, pad_idx=1):
         return R.text_embed_ref(tokens, table, pos, cls, pad_idx)
@@ -198,6 +205,102 @@ class Emu:
         x.view(-1, x.shape[-1])[pad_mask.reshape(-1).bool()] = 0
         return x
 
+    # the classification heads and criteria (csrc/classify.cu, vit_head.cu, grounding.cu): their fp64 references
+    def attn_pool_fwd(self, kv, q, key_pad, B, T):
+        out, lse, _, _ = CH.pool_fwd_ref(kv, q, key_pad, B, T)
+        return out.to(BF), lse.float()
+
+    def attn_pool_bwd(self, kv, q, key_pad, lse, dout, B, T):
+        dkv, dq, _, _ = CH.pool_bwd_ref(kv, q, key_pad, dout, B, T)
+        return dkv.to(BF), dq.float()
+
+    def classify_loss(self, logits, n_valid, mode, labels=None, targets=None, eps=0.0, num_choices=1):
+        r = CH.loss_ref(logits, n_valid, mode, labels=labels, targets=targets, eps=eps, num_choices=num_choices)
+        dl = torch.full((logits.shape[0], logits.stride(0)), float("nan"))      # columns past n_valid are not defined
+        dl[:, :r["dlogits"].shape[1]] = r["dlogits"].float()
+        return r["row_loss"].float(), dl, r["row_correct"].float(), torch.stack([r["loss"], r["n_correct"]]).float()
+
+    def refcoco_loss(self, logits, targets, nsentences):
+        with torch.enable_grad():                          # refcoco's bounds are taken by autograd
+            r = refcoco(logits, targets, nsentences)
+        dl = torch.full((logits.shape[0], logits.stride(0)), float("nan"))
+        dl[:, :4] = r["dlogits"].float()
+        out = torch.tensor([float(r["loss"]), float(r["l1"]), float(r["n_valid"])])
+        return out, r["valid"].int(), r["giou"].float(), dl
+
+    def token_mean_ln_fwd(self, x, gamma, beta, eps):
+        f = head_fwd(x, gamma, beta, eps)
+        return f["y"].to(BF), f["m"].float(), f["mean"].float(), f["rstd"].float()
+
+    def token_mean_ln_bwd(self, dy, m, mean, rstd, gamma, dx):
+        hb = head_bwd(dy, m, mean, rstd, gamma, dx.shape[1])
+        dx.copy_(hb["dx"])
+        return hb["dgamma"].float(), hb["dbeta"].float()
+
+    # the pretraining path: gathers, bias blocks, the DCL loss's InfoNCE
+    def row_gather(self, src, idx, out=None, fill=None, out_dtype=None, add=None):
+        rows, dim = idx.numel(), src.shape[1]
+        if out is None:
+            out = torch.empty(rows, dim, dtype=out_dtype or src.dtype)
+        v = torch.where((idx >= 0)[:, None], src.double()[idx.clamp_min(0)], fill.double() if fill is not None else 0.0)
+        if add is not None:
+            a = add.reshape(-1, dim).double()
+            v = v + a[torch.arange(rows) % a.shape[0]]
+        out.copy_(v.to(out.dtype))
+        return out
+
+    def row_scatter_add(self, dout, idx, dsrc):
+        keep = idx >= 0
+        if self.scatter_overwrite:
+            dsrc[idx[keep]] = dout[keep].to(dsrc.dtype)
+        else:
+            dsrc.copy_(dsrc.double().index_add(0, idx[keep], dout.double()[keep]))
+        return dsrc
+
+    def relpos_bias_block(self, table, bucket, ids, n, lo, bias, S, H):
+        bias.copy_(R.relpos_bias_block_ref(table, bucket, ids, n, lo, bias)[0])
+        return bias
+
+    def relpos_bias_block_bwd(self, dbias, bucket, ids, n, lo, dtable, S, H):
+        Bb = dbias.shape[0]
+        p = torch.arange(n).expand(Bb, n) if ids is None else torch.where(ids < 0, n - 1, ids)
+        dest = bucket[p[:, :, None], p[:, None, :]].reshape(-1)
+        src = dbias[:, :, lo:lo + n, lo:lo + n].double().permute(0, 2, 3, 1).reshape(-1, H)
+        dtable.copy_(dtable.double().index_add(0, dest, src))
+        return dtable
+
+    def split_bf16x3(self, xs, sides):
+        outs = []
+        for x, side in zip(xs, sides):
+            hi = x.to(BF)
+            lo = (x - hi.float()).to(BF)
+            outs.append(torch.cat([hi, hi, lo] if side == 0 else [hi, lo, hi], 1))
+        return outs
+
+    @staticmethod
+    def _infonce(a3, b3, scale, n_valid, target_offset, eps):
+        """z = s a3 b3^T over the n class columns, the targets, the smoothing weights (kernel_ref.infonce_ref)"""
+        n = n_valid or b3.shape[0]
+        z = float(scale) * (a3.double() @ b3.double().t())[:, :n]
+        rows = torch.arange(z.shape[0])
+        eps_i = eps / (n - 1) if eps else 0.0
+        return z, rows, rows + target_offset, eps_i, 1.0 - eps - eps_i
+
+    def infonce_forward(self, pairs, scale, target_offset, eps, n_valid=0, rows=False):
+        ((a3, b3),) = pairs
+        assert not rows
+        z, r, tgt, eps_i, hit = self._infonce(a3, b3, scale, n_valid, target_offset, eps)
+        lse = torch.logsumexp(z, 1)
+        loss = hit * (lse - z[r, tgt]) + eps_i * (z.shape[1] * lse - z.sum(1))
+        out3 = torch.stack([loss.mean(), (z.argmax(1) == tgt).double().sum(), torch.zeros((), dtype=torch.float64)])
+        return [lse.float()], out3.float()
+
+    def infonce_grad(self, a_local, b_all, scale, row_lse, target_offset, eps, d, n_valid=0, coef=0.0):
+        z, r, tgt, eps_i, hit = self._infonce(a_local, b_all, scale, n_valid, target_offset, eps)
+        G = (z - row_lse.double()[:, None]).exp() - eps_i
+        G[r, tgt] -= hit
+        return (float(scale) * coef * (G @ b_all[:z.shape[1], :d].double())).float(), None
+
 
 class Recorder:
     """Forwards every kernel call to ``kernels`` and logs (name, args, kwargs, result): the backward's intermediates are
@@ -218,16 +321,28 @@ class Recorder:
         return call
 
 
-def functions(kernels, edit=None):
-    """The Functions of a fresh copy of one_peace_b200/autograd.py whose kernels are ``kernels`` behind a ``Recorder``
-    (``.K``); edit = (old, new) replaces the one occurrence of ``old`` in its source."""
-    src = inspect.getsource(AG)
-    if edit is not None:
-        assert src.count(edit[0]) == 1, edit[0]
-        src = src.replace(*edit)
-    ns = {"__name__": "one_peace_b200._stem_emulated", "__package__": "one_peace_b200"}
-    exec(compile(src, AG.__file__, "exec"), ns)
-    ns["K"] = Recorder(kernels)
+def functions(kernels, edit=None, module=AG):
+    """The Functions of a fresh copy of ``module`` (one_peace_b200/autograd.py by default) whose kernels are ``kernels``
+    behind a ``Recorder`` (``.K``); edit = (old, new) replaces the one occurrence of ``old`` in its source.  What the
+    module imports from autograd (``_dw``, ``_dx``, ``_pad8``) is taken from a fresh copy of autograd on the same Recorder,
+    so that those helpers' GEMMs and transposes also run on ``kernels`` and appear in the log."""
+    rec = Recorder(kernels)
+
+    def fresh(mod, ed):
+        src = inspect.getsource(mod)
+        if ed is not None:
+            assert src.count(ed[0]) == 1, ed[0]
+            src = src.replace(*ed)
+        ns = {"__name__": mod.__name__ + "_emulated", "__package__": "one_peace_b200"}
+        exec(compile(src, mod.__file__, "exec"), ns)
+        ns["K"] = rec
+        return ns
+    ns = fresh(module, edit)
+    if module is not AG:
+        ag = fresh(AG, None)
+        for k, v in ns.items():
+            if k != "K" and getattr(AG, k, None) is v:
+                ns[k] = ag[k]
     return SimpleNamespace(**ns)
 
 
