@@ -60,6 +60,10 @@ OPB_DEVICE void mbar_arrive_expect_tx(uint64_t* bar, uint32_t bytes) {
 OPB_DEVICE void mbar_arrive(uint64_t* bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
+// one thread arriving on behalf of `count` (e.g. every warp of its warpgroup)
+OPB_DEVICE void mbar_arrive_count(uint64_t* bar, uint32_t count) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
+}
 OPB_DEVICE bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
   uint32_t ok;
   asm volatile(

@@ -13,6 +13,9 @@
 //     quad.  gemm_bf16_kernel stores the results straight to global memory.  gemm_bf16_tma_out_kernel (the bf16 epilogues on
 //     a plain row-major output) writes them with stmatrix into a per-warpgroup shared-memory copy of its 64 output rows and
 //     one thread hands that to TMA bulk stores, so the stores drain while the warpgroup runs the next tile's mainloop.
+//     gemm_bf16_resid_tma_kernel (the residual epilogue on plain aligned operands) has the producer load the fp32 residual
+//     into the stage ring after the tile's k-blocks, 64 columns per stage, and stores each chunk's fp32 result and bf16
+//     copy from that stage with TMA (see epilogue_resid_ring).
 //
 // Fused epilogues (what the reference runs as separate ATen kernels, SURVEY.md 2.5 K1'/K3/K4):
 //   EPI_STORE_BF16 : out_bf16 = (acc + bias[n]) * colscale[n]        (q/k/v projection, q pre-scaled;
@@ -65,6 +68,13 @@ constexpr int smem_bytes(int stages, bool tma_out) {
 constexpr int kSmemBytes = smem_bytes(kStages, false);
 constexpr int kSmemBytesTmaOut = smem_bytes(kStagesTmaOut, true);
 static_assert(kSmemBytesTmaOut <= 227 * 1024, "output staging does not fit next to the stage ring");
+// Residual chunks of gemm_bf16_resid_tma_kernel: a stage holds 64 columns of the tile's 128 rows, the fp32 residual (then
+// result) as two 32-column boxes of 16 KB and the bf16 copy as one 64-column box after them, all with the 128-byte swizzle.
+// A consumer warpgroup's 64 rows are the second half of each box (8 KB in).
+constexpr int kChunks = kBlockN / 64;
+constexpr int kResidBoxBytes = kBlockM * 128;
+constexpr int kChunkBf16Offset = 2 * kResidBoxBytes;
+static_assert(kChunkBf16Offset + kBlockM * 128 == kStageBytes, "a residual chunk fills one stage");
 
 struct GemmGeom {
   int M, N, K;          // per group: rows, output columns, reduction length (= taps * kb_inner * 64 when windowed)
@@ -480,6 +490,97 @@ OPB_DEVICE void epilogue(const float (&d)[128], const GemmEpilogue& ep, const Ge
   }
 }
 
+// EPI_RESID_F32 through the stage ring (gemm_bf16_resid_tma_kernel).  The producer follows the tile's k-blocks with kChunks
+// ring entries, entry it + c holding the residual of tile columns 64 c .. 64 c + 63 (rows >= M and columns >= N zero-filled).
+// For each chunk the warpgroup computes its 64 rows with the operations of epilogue<EPI_RESID_F32>, in the same order (st_sum
+// / st_sq run over the columns left to right across the chunks), writes the fp32 result over the residual it read and the
+// bf16 copy next to it, and one thread stores both with TMA as one bulk group (rows >= M and columns >= N clipped).  A
+// chunk's stage goes back to the producer once the stores of both warpgroups have read it: chunk c - 1 after chunk c's stores
+// are issued, the last chunk before the warpgroup leaves.  That is required, not only early: the next tile's first k-blocks
+// land in these stages, so a stage still held when the consumers wait on the next tile's `full` barriers would never fill.
+template <int S>
+OPB_DEVICE void epilogue_resid_ring(const float (&d)[128], const GemmEpilogue& ep, const GemmGeom& geo, const EpiOperands* st,
+                                    uint8_t* smem, uint64_t* full, uint64_t* empty, const CUtensorMap& tm_out,
+                                    const CUtensorMap& tm_out_bf16, uint32_t it, int m_blk, int n_blk, int cw) {
+  const int M = geo.M, N = geo.N;
+  const int t = threadIdx.x & 127;
+  const int lane = t & 31;
+  const int quad = lane & 3;
+  const int rloc = cw * 64 + (t >> 5) * 16 + (lane >> 2);   // row inside the tile and the chunk's boxes (fragment row r)
+  const int rbase = m_blk * kBlockM + rloc;
+  const int row0 = m_blk * kBlockM + cw * 64;                // first row of the warpgroup's stores
+  const bool has_ln = ep.ln_colsum != nullptr;
+  const bool has_rows = ep.ln_partial != nullptr || ep.ln_mu != nullptr;
+  float st_sum[2] = {0.f, 0.f}, st_sq[2] = {0.f, 0.f};   // partial statistics of the stored values (next LayerNorm)
+#pragma unroll
+  for (int c = 0; c < kChunks; ++c) {
+    const uint32_t s = (it + c) % S;
+    mbar_wait_quiet(&full[s], ((it + c) / S) & 1);
+    uint8_t* stage = smem + s * kStageBytes;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {       // fragment rows r and r + 8
+      const int r = rloc + 8 * h;
+      const bool row_ok = rbase + 8 * h < M;
+      const float2 mr = has_rows ? st->row[r] : make_float2(0.f, 1.f);
+      const float mu = mr.x, rs = mr.y;
+#pragma unroll
+      for (int jj = 0; jj < 8; ++jj) {
+        const int j = 8 * c + jj;                  // column group of the fragment
+        const int lc = 8 * j + 2 * quad;           // column inside the tile
+        float2* f = reinterpret_cast<float2*>(stage + (jj >> 2) * kResidBoxBytes + sw128_off(r, 2 * (jj & 3) + (quad >> 1)) +
+                                              8 * (quad & 1));
+        float x0 = d[4 * j + 2 * h], x1 = d[4 * j + 2 * h + 1];
+        if (has_ln) {
+          const float2 cs = ldf2(st->colsum + lc);
+          x0 = rs * (x0 - mu * cs.x); x1 = rs * (x1 - mu * cs.y);
+        }
+        if (ep.bias != nullptr) {
+          const float2 b = ldf2(st->bias + lc);
+          x0 += b.x; x1 += b.y;
+        }
+        if (ep.gamma != nullptr) {
+          const float2 g = ldf2(st->gamma + lc);
+          x0 *= g.x; x1 *= g.y;
+        }
+        if (row_ok) {
+          const float2 res = *f;
+          x0 += res.x; x1 += res.y;
+        }
+        st_sum[h] += x0 + x1;
+        st_sq[h] += x0 * x0 + x1 * x1;
+        *f = make_float2(x0, x1);
+        *reinterpret_cast<uint32_t*>(stage + kChunkBf16Offset + sw128_off(r, jj) + 4 * quad) = pack_bf16x2(x0, x1);
+      }
+    }
+    fence_proxy_async();
+    warpgroup_bar_sync(cw);
+    if (t == 0) {
+      const int col = n_blk * kBlockN + 64 * c;
+      if (row0 < M) {
+        for (int b = 0; b < 2; ++b)
+          if (col + 32 * b < N) tma_store_2d(&tm_out, stage + b * kResidBoxBytes + cw * 64 * 128, col + 32 * b, row0);
+        if (ep.out_bf16 != nullptr && col < N) tma_store_2d(&tm_out_bf16, stage + kChunkBf16Offset + cw * 64 * 128, col, row0);
+      }
+      bulk_commit();
+      if (c > 0) {                     // the stores of chunk c - 1 have read their stage
+        bulk_wait_read<1>();
+        mbar_arrive_count(&empty[(it + c - 1) % S], 4);
+      }
+      if (c == kChunks - 1) {
+        bulk_wait_read<0>();
+        mbar_arrive_count(&empty[s], 4);
+      }
+    }
+  }
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int row = rbase + 8 * h;
+    const float s1 = quad_sum(st_sum[h]), s2 = quad_sum(st_sq[h]);
+    if (row < M && quad == 0 && ep.stats_out != nullptr)
+      *reinterpret_cast<float2*>(ep.stats_out + (static_cast<long>(n_blk) * M + row) * 2) = make_float2(s1, s2);
+  }
+}
+
 // Work unit -> tile.  Units are split-K piece-major (a single piece unless split-K), then group-major; inside a group the
 // tiles run in bands of kBandM row panels, row panel fastest.
 struct TileCoord {
@@ -501,12 +602,19 @@ OPB_DEVICE TileCoord tile_coord(int unit, int num_m_tiles, int num_n_tiles, int 
   return c;
 }
 
+// How a kernel's epilogue results leave the SM: stored from registers (gemm_bf16_kernel), staged bf16 tile and TMA stores
+// (gemm_bf16_tma_out_kernel), or the residual epilogue's chunks through the stage ring (gemm_bf16_resid_tma_kernel).
+enum class OutPath { kDirect, kTmaBf16, kResidRing };
+
 // Persistent: the grid holds as many CTAs as can be resident and CTA b runs units b, b + gridDim.x, ...  Barrier set-up and
-// descriptor prefetch happen once per CTA.  The body of both kernels: S pipeline stages; kTmaOut stages the bf16 output tile
-// in shared memory and stores it with TMA through tm_out (not used otherwise).
-template <int EPI, int S, bool kTmaOut>
-OPB_DEVICE void gemm_body(const CUtensorMap& tm_a, const CUtensorMap& tm_b, const CUtensorMap* tm_out, const GemmEpilogue& ep,
-                          const GemmGeom& geo) {
+// descriptor prefetch happen once per CTA.  The body of the three kernels: S pipeline stages; kTmaBf16 stages the bf16 output
+// tile in shared memory and stores it with TMA through tm_out; kResidRing loads the residual through tm_res into the stage
+// ring and stores through tm_out (fp32) and tm_out_bf16 (see epilogue_resid_ring).  Maps a path does not use are null.
+template <int EPI, int S, OutPath kPath>
+OPB_DEVICE void gemm_body(const CUtensorMap& tm_a, const CUtensorMap& tm_b, const CUtensorMap* tm_out, const CUtensorMap* tm_res,
+                          const CUtensorMap* tm_out_bf16, const GemmEpilogue& ep, const GemmGeom& geo) {
+  constexpr bool kTmaOut = kPath == OutPath::kTmaBf16;
+  constexpr bool kRing = kPath == OutPath::kResidRing;
   // no static shared memory: the dynamic window starts at the 1024-aligned base the 128-byte swizzle needs (checked)
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = smem_raw;
@@ -525,12 +633,16 @@ OPB_DEVICE void gemm_body(const CUtensorMap& tm_a, const CUtensorMap& tm_b, cons
   const int pieces = geo.kb_per_piece > 0 ? (geo.num_k_blocks + geo.kb_per_piece - 1) / geo.kb_per_piece : 1;
   const int units = num_m_tiles * num_n_tiles * geo.groups * pieces;
   // split-K pieces store raw accumulators and need no epilogue operands
-  const bool staged = epi_staged(EPI) && (kTmaOut || geo.kb_per_piece == 0);
+  const bool staged = epi_staged(EPI) && (kTmaOut || kRing || geo.kb_per_piece == 0);
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tm_a);
     tma_prefetch_desc(&tm_b);
-    if constexpr (kTmaOut) tma_prefetch_desc(tm_out);
+    if constexpr (kTmaOut || kRing) tma_prefetch_desc(tm_out);
+    if constexpr (kRing) {
+      tma_prefetch_desc(tm_res);
+      if (ep.out_bf16 != nullptr) tma_prefetch_desc(tm_out_bf16);
+    }
     for (int i = 0; i < S; ++i) {
       mbar_init(&full[i], 1);
       mbar_init(&empty[i], 8);   // lane 0 of each of the 8 consumer warps
@@ -576,6 +688,17 @@ OPB_DEVICE void gemm_body(const CUtensorMap& tm_a, const CUtensorMap& tm_b, cons
           }
           if (++kin == geo.kb_inner) { kin = 0; ++tap; }
         }
+        if constexpr (kRing) {
+          // the tile's residual, kChunks ring entries of 64 columns (see epilogue_resid_ring)
+          for (int c = 0; c < kChunks; ++c, ++it) {
+            const uint32_t s = it % S;
+            mbar_wait_quiet(&empty[s], ((it / S) & 1) ^ 1);
+            uint8_t* sr = smem + s * kStageBytes;
+            mbar_arrive_expect_tx(&full[s], 2 * kResidBoxBytes);
+            for (int b = 0; b < 2; ++b)
+              tma_load_2d(tm_res, &full[s], sr + b * kResidBoxBytes, tc.n_blk * kBlockN + 64 * c + 32 * b, a_row);
+          }
+        }
       }
     } else if (threadIdx.x >= 32 && staged) {
       // ===================== epilogue-operand stager (warps 1-3) =====================
@@ -608,7 +731,7 @@ OPB_DEVICE void gemm_body(const CUtensorMap& tm_a, const CUtensorMap& tm_b, cons
         else mainloop<0, 0, S>(d, smem, full, empty, kb1 - kb0, cw, it);
       }
       it += kb1 - kb0;
-      if (!kTmaOut && geo.kb_per_piece > 0) {   // (the staged-output kernel never runs split-K)
+      if (kPath == OutPath::kDirect && geo.kb_per_piece > 0) {   // (the TMA-store kernels never run split-K)
         // split-K piece: raw partial accumulators of all m_pad rows into this piece's slab (plain stores, no atomics)
         const int t = threadIdx.x & 127, lane = t & 31;
         const int r0 = tc.m_blk * kBlockM + cw * 64 + (t >> 5) * 16 + (lane >> 2);
@@ -625,7 +748,12 @@ OPB_DEVICE void gemm_body(const CUtensorMap& tm_a, const CUtensorMap& tm_b, cons
       } else if (staged) {
         mbar_wait_quiet(&epi_full[j & 1], (j >> 1) & 1);
         if constexpr (kTmaOut) acquire_out_stage(cw);
-        epilogue<EPI, kTmaOut>(d, ep, geo, &epi_ops[j & 1], smem_u32(my_stage), tc.m_blk, tc.n_blk, tc.grp, cw);
+        if constexpr (kRing) {
+          epilogue_resid_ring<S>(d, ep, geo, &epi_ops[j & 1], smem, full, empty, *tm_out, *tm_out_bf16, it, tc.m_blk, tc.n_blk, cw);
+          it += kChunks;
+        } else {
+          epilogue<EPI, kTmaOut>(d, ep, geo, &epi_ops[j & 1], smem_u32(my_stage), tc.m_blk, tc.n_blk, tc.grp, cw);
+        }
         __syncwarp();
         if ((threadIdx.x & 31) == 0) mbar_arrive(&epi_empty[j & 1]);
         if constexpr (kTmaOut) {
@@ -639,7 +767,7 @@ OPB_DEVICE void gemm_body(const CUtensorMap& tm_a, const CUtensorMap& tm_b, cons
       }
     }
     // the staging area must outlive the last bulk stores
-    if constexpr (kTmaOut) {
+    if constexpr (kTmaOut || kRing) {
       if ((threadIdx.x & 127) == 0) bulk_wait_all<0>();
     }
   }
@@ -649,7 +777,7 @@ template <int EPI>
 __global__ void __launch_bounds__(kThreads, 1)
 gemm_bf16_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__ CUtensorMap tm_b, const GemmEpilogue ep,
                  const GemmGeom geo) {
-  gemm_body<EPI, kStages, false>(tm_a, tm_b, nullptr, ep, geo);
+  gemm_body<EPI, kStages, OutPath::kDirect>(tm_a, tm_b, nullptr, nullptr, nullptr, ep, geo);
 }
 
 // The bf16 epilogues with the output tile staged in shared memory and stored by TMA through tm_out (rows M, columns N, or
@@ -660,7 +788,20 @@ __global__ void __launch_bounds__(kThreads, 1)
 gemm_bf16_tma_out_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__ CUtensorMap tm_b,
                          const __grid_constant__ CUtensorMap tm_out, const GemmEpilogue ep, const GemmGeom geo) {
   static_assert(EPI == EPI_STORE_BF16 || EPI == EPI_GELU_BF16 || EPI == EPI_GEGLU_BF16, "bf16 epilogues only");
-  gemm_body<EPI, kStagesTmaOut, true>(tm_a, tm_b, &tm_out, ep, geo);
+  gemm_body<EPI, kStagesTmaOut, OutPath::kTmaBf16>(tm_a, tm_b, &tm_out, nullptr, nullptr, ep, geo);
+}
+
+// EPI_RESID_F32 with the residual loaded into the stage ring by TMA through tm_res (fp32 [M, N], box 32 x 128) and the results
+// stored by TMA through tm_out (fp32 [M, N], box 32 x 64) and tm_out_bf16 (bf16 [M, N], box 64 x 64; unused without
+// out_bf16), all with the 128-byte swizzle.  Four stages and no shared memory beyond gemm_bf16_kernel's.  Taken only for a
+// single group, no split-K, no row remapping or residual period, and 16-byte aligned operands (see resid_ring_applies).
+template <int EPI>
+__global__ void __launch_bounds__(kThreads, 1)
+gemm_bf16_resid_tma_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__ CUtensorMap tm_b,
+                           const __grid_constant__ CUtensorMap tm_res, const __grid_constant__ CUtensorMap tm_out,
+                           const __grid_constant__ CUtensorMap tm_out_bf16, const GemmEpilogue ep, const GemmGeom geo) {
+  static_assert(EPI == EPI_RESID_F32, "the residual epilogue only");
+  gemm_body<EPI, kStages, OutPath::kResidRing>(tm_a, tm_b, &tm_out, &tm_res, &tm_out_bf16, ep, geo);
 }
 
 // Epilogue of the small-M split-K schedule: x = sum of the piece slabs (fixed order), then the EPI_RESID_F32 epilogue
@@ -758,6 +899,21 @@ int make_tmap_bf16_2d(CUtensorMap* out, const void* ptr, uint64_t rows, uint64_t
   return r == CUDA_SUCCESS ? OPB_OK : OPB_ERR_CUDA;
 }
 
+// 2D fp32 row-major [rows, cols] with row pitch ld (elements); box = 32 cols (128 bytes) x box_rows, 128B swizzle.
+static int make_tmap_f32_2d(CUtensorMap* out, const void* ptr, uint64_t rows, uint64_t cols, uint64_t ld, uint32_t box_rows) {
+  PFN_encodeTiled enc = get_encode_fn();
+  if (enc == nullptr) return OPB_ERR_CUDA;
+  if ((reinterpret_cast<uintptr_t>(ptr) & 15) != 0 || (ld * 4) % 16 != 0) return OPB_ERR_INVALID;
+  cuuint64_t gdim[2] = {cols, rows};
+  cuuint64_t gstride[1] = {ld * 4};
+  cuuint32_t box[2] = {32, box_rows};
+  cuuint32_t estr[2] = {1, 1};
+  CUresult r = enc(out, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<void*>(ptr), gdim, gstride, box, estr,
+                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  return r == CUDA_SUCCESS ? OPB_OK : OPB_ERR_CUDA;
+}
+
 // 3D view of the A operand: dims {k_inner, taps, rows}; element (c, j, r) lives at ptr + r*row_stride + j*tap_stride + c.
 // A plain [rows, K] matrix is the taps == 1 case.  box = 64 x 1 x box_rows, 128B swizzle (same smem image as 2D).
 int make_tmap_bf16_3d(CUtensorMap* out, const void* ptr, uint64_t k_inner, uint64_t taps, uint64_t tap_stride,
@@ -795,13 +951,16 @@ int make_tmap_bf16_batched(CUtensorMap* out, const void* ptr, uint64_t cols, uin
   return r == CUDA_SUCCESS ? OPB_OK : OPB_ERR_CUDA;
 }
 
-// kTmaOut: gemm_bf16_tma_out_kernel<EPI> with the output tensor map `to`; otherwise gemm_bf16_kernel<EPI> (`to` unused)
-template <int EPI, bool kTmaOut>
+// The kernel of path kPath.  `to` holds its tensor maps: none (kDirect), the bf16 output (kTmaBf16), or the residual, the
+// fp32 output and the bf16 copy (kResidRing).
+template <int EPI, OutPath kPath>
 static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap* to, const GemmEpilogue& ep,
                        const GemmGeom& geo, cudaStream_t stream) {
+  constexpr bool kTmaOut = kPath == OutPath::kTmaBf16;
   constexpr int smem = kTmaOut ? kSmemBytesTmaOut : kSmemBytes;
   const void* kern;
   if constexpr (kTmaOut) kern = reinterpret_cast<const void*>(gemm_bf16_tma_out_kernel<EPI>);
+  else if constexpr (kPath == OutPath::kResidRing) kern = reinterpret_cast<const void*>(gemm_bf16_resid_tma_kernel<EPI>);
   else kern = reinterpret_cast<const void*>(gemm_bf16_kernel<EPI>);
   static int resident = 0;   // CTAs resident at once over the whole GPU
   if (resident == 0) {
@@ -815,30 +974,35 @@ static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, const CUten
   const int pieces = geo.kb_per_piece > 0 ? (geo.num_k_blocks + geo.kb_per_piece - 1) / geo.kb_per_piece : 1;
   const long units = static_cast<long>((geo.M + kBlockM - 1) / kBlockM) * ((geo.N + kBlockN - 1) / kBlockN) * geo.groups * pieces;
   const unsigned grid = static_cast<unsigned>(units < resident ? units : resident);
-  if constexpr (kTmaOut) gemm_bf16_tma_out_kernel<EPI><<<grid, kThreads, smem, stream>>>(ta, tb, *to, ep, geo);
+  if constexpr (kTmaOut) gemm_bf16_tma_out_kernel<EPI><<<grid, kThreads, smem, stream>>>(ta, tb, to[0], ep, geo);
+  else if constexpr (kPath == OutPath::kResidRing)
+    gemm_bf16_resid_tma_kernel<EPI><<<grid, kThreads, smem, stream>>>(ta, tb, to[0], to[1], to[2], ep, geo);
   else gemm_bf16_kernel<EPI><<<grid, kThreads, smem, stream>>>(ta, tb, ep, geo);
   return cudaGetLastError() == cudaSuccess ? OPB_OK : OPB_ERR_CUDA;
 }
 
-// `to` != nullptr: the output tensor map of the TMA-store kernel (bf16 epilogues only, see tma_out_applies)
+// `to` != nullptr: the tensor maps of the TMA-store kernels (the bf16 output for the bf16 epilogues, see tma_out_applies;
+// the residual, fp32 output and bf16 copy for EPI_RESID_F32, see resid_ring_applies)
 static int dispatch_gemm(int epi, const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap* to, const GemmEpilogue& ep,
                          const GemmGeom& geo, cudaStream_t stream) {
+  constexpr OutPath D = OutPath::kDirect, T = OutPath::kTmaBf16;
   if (to != nullptr) {
     switch (epi) {
-      case EPI_STORE_BF16: return launch_gemm<EPI_STORE_BF16, true>(ta, tb, to, ep, geo, stream);
-      case EPI_GELU_BF16: return launch_gemm<EPI_GELU_BF16, true>(ta, tb, to, ep, geo, stream);
-      case EPI_GEGLU_BF16: return launch_gemm<EPI_GEGLU_BF16, true>(ta, tb, to, ep, geo, stream);
+      case EPI_STORE_BF16: return launch_gemm<EPI_STORE_BF16, T>(ta, tb, to, ep, geo, stream);
+      case EPI_GELU_BF16: return launch_gemm<EPI_GELU_BF16, T>(ta, tb, to, ep, geo, stream);
+      case EPI_GEGLU_BF16: return launch_gemm<EPI_GEGLU_BF16, T>(ta, tb, to, ep, geo, stream);
+      case EPI_RESID_F32: return launch_gemm<EPI_RESID_F32, OutPath::kResidRing>(ta, tb, to, ep, geo, stream);
       default: return OPB_ERR_INVALID;
     }
   }
   switch (epi) {
-    case EPI_STORE_BF16: return launch_gemm<EPI_STORE_BF16, false>(ta, tb, nullptr, ep, geo, stream);
-    case EPI_GELU_BF16: return launch_gemm<EPI_GELU_BF16, false>(ta, tb, nullptr, ep, geo, stream);
-    case EPI_GEGLU_BF16: return launch_gemm<EPI_GEGLU_BF16, false>(ta, tb, nullptr, ep, geo, stream);
-    case EPI_RESID_F32: return launch_gemm<EPI_RESID_F32, false>(ta, tb, nullptr, ep, geo, stream);
-    case EPI_STORE_F32: return launch_gemm<EPI_STORE_F32, false>(ta, tb, nullptr, ep, geo, stream);
-    case EPI_LSE_PARTIAL: return launch_gemm<EPI_LSE_PARTIAL, false>(ta, tb, nullptr, ep, geo, stream);
-    case EPI_SOFTMAX_GRAD: return launch_gemm<EPI_SOFTMAX_GRAD, false>(ta, tb, nullptr, ep, geo, stream);
+    case EPI_STORE_BF16: return launch_gemm<EPI_STORE_BF16, D>(ta, tb, nullptr, ep, geo, stream);
+    case EPI_GELU_BF16: return launch_gemm<EPI_GELU_BF16, D>(ta, tb, nullptr, ep, geo, stream);
+    case EPI_GEGLU_BF16: return launch_gemm<EPI_GEGLU_BF16, D>(ta, tb, nullptr, ep, geo, stream);
+    case EPI_RESID_F32: return launch_gemm<EPI_RESID_F32, D>(ta, tb, nullptr, ep, geo, stream);
+    case EPI_STORE_F32: return launch_gemm<EPI_STORE_F32, D>(ta, tb, nullptr, ep, geo, stream);
+    case EPI_LSE_PARTIAL: return launch_gemm<EPI_LSE_PARTIAL, D>(ta, tb, nullptr, ep, geo, stream);
+    case EPI_SOFTMAX_GRAD: return launch_gemm<EPI_SOFTMAX_GRAD, D>(ta, tb, nullptr, ep, geo, stream);
     default: return OPB_ERR_INVALID;
   }
 }
@@ -850,6 +1014,21 @@ static int dispatch_gemm(int epi, const CUtensorMap& ta, const CUtensorMap& tb, 
 static bool tma_out_applies(int epi, const GemmEpilogue& ep, const GemmGeom& geo, long out_cols) {
   return (epi == EPI_STORE_BF16 || epi == EPI_GELU_BF16 || epi == EPI_GEGLU_BF16) && geo.kb_per_piece == 0 && geo.groups == 1 &&
          ep.out_group == 0 && (reinterpret_cast<uintptr_t>(ep.out) & 15) == 0 && (ep.ldo * 2) % 16 == 0 && ep.ldo >= out_cols;
+}
+
+// EPI_RESID_F32 loads its residual into the stage ring and stores its results with TMA (gemm_bf16_resid_tma_kernel) when the
+// residual, the fp32 output and the bf16 copy (if any) are each one plain row-major [M, N] matrix a tensor map can describe:
+// no split-K, one group, no row remapping, no residual period, 16-byte aligned bases and row pitches, pitches no smaller than
+// the row.  Every other call (the small-M split-K path, the adapters' remapped rows, misaligned operands) keeps
+// gemm_bf16_kernel.  Updating the residual in place (resid == out) is safe: a chunk is loaded whole before any of it is
+// stored, and tiles are disjoint.
+static bool resid_ring_applies(int epi, const GemmEpilogue& ep, const GemmGeom& geo) {
+  auto plain = [&](const void* p, long ld, int esz) {
+    return (reinterpret_cast<uintptr_t>(p) & 15) == 0 && (ld * esz) % 16 == 0 && ld >= geo.N;
+  };
+  return epi == EPI_RESID_F32 && geo.kb_per_piece == 0 && geo.groups == 1 && ep.out_group == 0 && ep.resid_period == 0 &&
+         ep.resid != nullptr && plain(ep.resid, ep.ldr, 4) && plain(ep.out, ep.ldo, 4) &&
+         (ep.out_bf16 == nullptr || plain(ep.out_bf16, ep.ldo_bf16, 2));
 }
 
 // Bytes [begin, end) spanned by rows lo..hi of a row-major matrix with pitch ld and `cols` columns of `esz` bytes.
@@ -940,10 +1119,17 @@ int gemm_bf16(const void* A, int lda, const void* B, int ldb, int M, int N, int 
   rc = make_tmap_bf16_2d(&tb, B, N, K, ldb, kBlockN);
   if (rc != OPB_OK) return rc;
   const long out_cols = epi == EPI_GEGLU_BF16 ? N / 2 : N;
-  CUtensorMap to;
+  CUtensorMap to[3];
   const bool tma_out = tma_out_applies(epi, ep, geo, out_cols);
-  if (tma_out && (rc = make_tmap_bf16_2d(&to, ep.out, M, out_cols, ep.ldo, 64)) != OPB_OK) return rc;
-  rc = dispatch_gemm(epi, ta, tb, tma_out ? &to : nullptr, ep, geo, stream);
+  const bool ring = resid_ring_applies(epi, ep, geo);
+  if (tma_out && (rc = make_tmap_bf16_2d(&to[0], ep.out, M, out_cols, ep.ldo, 64)) != OPB_OK) return rc;
+  if (ring) {
+    if ((rc = make_tmap_f32_2d(&to[0], ep.resid, M, N, ep.ldr, kBlockM)) != OPB_OK) return rc;
+    if ((rc = make_tmap_f32_2d(&to[1], ep.out, M, N, ep.ldo, 64)) != OPB_OK) return rc;
+    to[2] = to[1];   // (not read without a bf16 copy)
+    if (ep.out_bf16 != nullptr && (rc = make_tmap_bf16_2d(&to[2], ep.out_bf16, M, N, ep.ldo_bf16, 64)) != OPB_OK) return rc;
+  }
+  rc = dispatch_gemm(epi, ta, tb, tma_out || ring ? to : nullptr, ep, geo, stream);
   if (rc != OPB_OK || geo.kb_per_piece == 0) return rc;
   gemm_split_epilogue_kernel<<<dim3(M, n_tiles), 256, 0, stream>>>(ep, geo, pieces, epi);
   return cudaGetLastError() == cudaSuccess ? OPB_OK : OPB_ERR_CUDA;
