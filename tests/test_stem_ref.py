@@ -7,7 +7,7 @@ gathers, strided rows).  The Functions run unchanged on it, packs, views and shi
 autograd module's source.  Their results must stay within the bounds, and each planted mistake (a one-line change of that
 source, or of one emulated kernel) must exceed them at least 100-fold somewhere.  tests/test_head_ref.py runs the
 classification heads, the criteria and the pretraining-path Functions on the same ``Emu``, ``Recorder`` and
-``functions``."""
+``functions``; tests/test_layer_ref.py runs the encoder stack on them."""
 import inspect
 from types import SimpleNamespace
 
@@ -27,29 +27,35 @@ MISS = 100.0            # a planted mistake must use at least this many times it
 
 
 class Emu:
-    """fp64 emulation of the kernels the training Functions around the encoder stack call (``one_peace_b200.kernels``
-    signatures).  Flags plant mistakes inside a kernel: ``text_pad_grad`` (padding tokens get a gradient),
+    """fp64 emulation of the kernels the training Functions call, around and inside the encoder stack
+    (``one_peace_b200.kernels`` signatures).  Flags plant mistakes inside a kernel: ``text_pad_grad`` (padding tokens get a gradient),
     ``text_pos_shift`` (position gradients one row early), ``l2_no_radial`` (l2-normalize backward without the radial
-    projection), ``scatter_overwrite`` (row_scatter_add stores instead of adding, so a repeated index keeps one row)."""
+    projection), ``scatter_overwrite`` (row_scatter_add stores instead of adding, so a repeated index keeps one row),
+    ``dbias_t_overwrite`` (attention_bwd_t stores its bias gradient into the transposed table instead of adding, so layers
+    that share a table keep only the last one's).  tests/test_layer_ref.py runs the encoder stack on it."""
     EPI_STORE_BF16, EPI_GEGLU_BF16, EPI_RESID_F32, EPI_STORE_F32, EPI_GELU_BF16 = 0, 1, 2, 3, 4
+    BIAS_T_KEYS, BIAS_T_Q = 256, 224        # the transposed bias tables of the attention backward
 
     def __init__(self, **flags):
         self.text_pad_grad = flags.pop("text_pad_grad", False)
         self.text_pos_shift = flags.pop("text_pos_shift", False)
         self.l2_no_radial = flags.pop("l2_no_radial", False)
         self.scatter_overwrite = flags.pop("scatter_overwrite", False)
+        self.dbias_t_overwrite = flags.pop("dbias_t_overwrite", False)
         assert not flags
 
     @staticmethod
     def _rows(t, rows, dim, ld):
         return t.as_strided((rows, dim), (ld, 1))
 
-    def gemm(self, a, w, epi, out, *, bias=None, out_group=0, out_group_stride=0, out_row_offset=0, resid=None,
-             resid_period=0, resid_row_offset=0, **kw):
+    def gemm(self, a, w, epi, out, *, bias=None, colscale=None, out_group=0, out_group_stride=0, out_row_offset=0,
+             resid=None, resid_period=0, resid_row_offset=0, **kw):
         assert not kw
         y = a.double() @ w.double().t()
         if bias is not None:
             y = y + bias.double()
+        if colscale is not None:
+            y = y * colscale.double()
         if epi == self.EPI_RESID_F32:
             N = y.shape[1]
             m = torch.arange(y.shape[0])
@@ -125,17 +131,27 @@ class Emu:
         return out
 
     def scale_resid_bwd(self, dx, o, gamma, row_scale, d_o, dgamma=None, dbias=None, in_period=0, in_valid=0, in_shift=0):
-        assert o is None and gamma is None and row_scale is None and dgamma is None
         rows, n = d_o.shape
-        v = dx.reshape(-1, n)[R.scale_resid_rows(rows, in_period, in_valid, in_shift)].double()
-        d_o.copy_(v.to(BF))
+        r = R.scale_resid_bwd_ref(dx.reshape(-1, n)[R.scale_resid_rows(rows, in_period, in_valid, in_shift)], o, gamma,
+                                  row_scale)
+        d_o.copy_(r.d_o.to(BF))
+        if dgamma is not None:
+            dgamma.copy_(r.dgamma)
         if dbias is not None:
-            dbias.copy_(v.sum(0))
+            dbias.copy_(r.dbias)
         return d_o
 
     def scale_resid_fwd(self, x, o, gamma, row_scale, out):
-        out.copy_(x.double() + o.double())
+        out.copy_(R.scale_resid_ref(x, o, gamma, row_scale)[0])
         return out
+
+    def geglu_fwd(self, gl, u):
+        u.copy_(R.geglu_ref(gl)[0])
+        return u
+
+    def geglu_bwd(self, gl, du, dgl):
+        dgl.copy_(R.geglu_bwd_ref(gl, du)[0])
+        return dgl
 
     def colsum(self, y, out):
         out.copy_(y.double().sum(0))
@@ -269,6 +285,55 @@ class Emu:
         dtable.copy_(dtable.double().index_add(0, dest, src))
         return dtable
 
+    # the encoder stack's attention (csrc/attention.cu, attention_bwd.cu): the fp64 references on the values the kernels read
+    def attention(self, qkv, bias, key_pad, B, S, H, out=None, lse=None, ln_stats=None):
+        assert ln_stats is None
+        f = R.attention_ref(qkv, None if bias is None else bias[..., :S], key_pad, B, S, H)
+        out.copy_(f.out)
+        if lse is not None:
+            lse.copy_(f.lse.reshape(-1))
+        return out
+
+    def attention_tc(self, qkv, rp, key_pad, B, S, H, out=None, ln_stats=None, lse=None):
+        assert not getattr(rp, "seg_split", 0)
+        dense = rp.lut[:, (rp.code_row[:S, None] - rp.code_col[None, :S]).long()]
+        return self.attention(qkv, dense, key_pad, B, S, H, out=out, lse=lse, ln_stats=ln_stats)
+
+    def attention_bwd(self, qkv, out, d_out, bias, key_pad, lse, dqkv, dbias, B, S, H, q_scale):
+        r = R.attention_bwd_ref(qkv, out, d_out, lse, None if bias is None else bias[..., :S], key_pad, B, S, H, q_scale)
+        dqkv.copy_(r.dqkv)
+        if dbias is not None:
+            d = dbias[..., :S]
+            d.copy_(d.double() + (r.dS if dbias.dim() == 4 else r.dS.sum(0)))
+        return dqkv
+
+    def relpos_bias_transpose(self, bias):
+        """(H,S,S_pad) -> (H,256,224) fp16(b log2 e), transposed, zero-padded, stored as (H,256,112) half2 words"""
+        H, S, _ = bias.shape
+        t = torch.zeros(H, self.BIAS_T_KEYS, self.BIAS_T_Q, dtype=torch.float16, device=bias.device)
+        t[:, :S, :S] = (bias[..., :S].float() * 1.4426950408889634).transpose(1, 2).half()
+        return t.view(torch.int32)
+
+    def attention_bwd_t(self, qkv, out, d_out, bias_t, key_pad, lse, dqkv, dbias_t, B, S, H, q_scale):
+        bias = bias_t.view(torch.float16)[:, :S, :S].transpose(1, 2).double() / 1.4426950408889634
+        r = R.attention_bwd_ref(qkv, out, d_out, lse, bias, key_pad, B, S, H, q_scale)
+        dqkv.copy_(r.dqkv)
+        d = dbias_t[:, :S, :S]
+        d.copy_(r.dS.sum(0).transpose(1, 2) + (0.0 if self.dbias_t_overwrite else d.double()))
+        return dqkv
+
+    def relpos_dbias_fold(self, dbias_t, dbias):
+        S = dbias.shape[1]
+        d = dbias[..., :S]
+        d.copy_(d.double() + dbias_t[:, :S, :S].double().transpose(1, 2))
+        return dbias
+
+    def relpos_dbias_center(self, dbias):
+        S = dbias.shape[1]
+        d = dbias[..., :S]
+        d.copy_(d.double() - d.double().mean(-1, keepdim=True))
+        return dbias
+
     def split_bf16x3(self, xs, sides):
         outs = []
         for x, side in zip(xs, sides):
@@ -321,12 +386,12 @@ class Recorder:
         return call
 
 
-def functions(kernels, edit=None, module=AG):
+def functions(kernels, edit=None, module=AG, recorder=Recorder):
     """The Functions of a fresh copy of ``module`` (one_peace_b200/autograd.py by default) whose kernels are ``kernels``
-    behind a ``Recorder`` (``.K``); edit = (old, new) replaces the one occurrence of ``old`` in its source.  What the
+    behind a ``recorder`` (``Recorder`` or a subclass; ``.K``); edit = (old, new) replaces the one occurrence of ``old`` in its source.  What the
     module imports from autograd (``_dw``, ``_dx``, ``_pad8``) is taken from a fresh copy of autograd on the same Recorder,
     so that those helpers' GEMMs and transposes also run on ``kernels`` and appear in the log."""
-    rec = Recorder(kernels)
+    rec = recorder(kernels)
 
     def fresh(mod, ed):
         src = inspect.getsource(mod)
