@@ -140,6 +140,20 @@ int opb_attention_decomp_fwd(const void* qkv, const float* lut, int lut_len, con
                              int H, void* stream);
 
 /*
+ * Temporal attention of the video backbone (one_peace_vision/video/mmaction_custom/models/backbones/onepeace.py:331-337 with
+ * num_tadapter = 1: rearrange 'n (b t) d -> t (b n) d', self_attn, rearrange back).  It replaces the reference's two
+ * rearranges and its bmm / softmax / bmm over Bv * N sequences of T frames.
+ *   qkv : bf16 [Bv * T * N, 3 * H * 64], frame-major rows (row (b * T + t) * N + n), q pre-scaled by head_dim^-0.5.
+ *   out : bf16 [Bv * T * N, H * 64], the same rows: out[(b, t, n), h] = softmax_t'(q_t . k_t') v_t' over the T frames of
+ *         (b, n), no bias, no padding.
+ *   ln_stats : fp32 [H, Bv * T * N, 2], opb_attention_fwd's per-(head, row) (sum, sum of squares) records of the fp32 output
+ *         values, for ln_partial = (ln_stats, H, H * 64, eps) of the out_proj GEMM.
+ * Needs 2 <= T <= 32, Bv, N, H >= 1, non-null 16-byte aligned qkv / out and an 8-byte aligned ln_stats; anything else
+ * returns OPB_ERR_INVALID before a launch.
+ */
+int opb_attention_temporal_fwd(const void* qkv, void* out, float* ln_stats, int Bv, int T, int N, int H, void* stream);
+
+/*
  * GEMM with the full epilogue description (superset of opb_gemm_bf16).  Adds the fused-LayerNorm form
  *   LN(x) W^T + b  =  rstd[m] * (acc - mu[m] * colsum[n]) + bias'[n]
  * where A holds the UN-normalised rows (bf16), B = W * diag(ln_weight) (bf16), colsum[n] = sum_k B[n,k],

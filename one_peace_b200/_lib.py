@@ -33,6 +33,7 @@ SIGNATURES = {
                                        c_int, c_int, c_int, c_int, c_void_p]),
     "opb_attention_decomp_fwd": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                          c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
+    "opb_attention_temporal_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
     "opb_gemm_bf16_ex": (c_int, [c_void_p, c_void_p]),
     "opb_row_stats_cast": (c_int, [c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_void_p, c_int, c_int, c_float, c_void_p]),
     "opb_ln_stats_finalize": (c_int, [c_void_p, c_int, c_int, c_int, c_float, c_void_p, c_void_p, c_void_p]),

@@ -59,6 +59,10 @@ int opb_attention_tc_fwd(const void* qkv, const float* lut, const float* lut_max
                                 static_cast<cudaStream_t>(stream));
 }
 
+int opb_attention_temporal_fwd(const void* qkv, void* out, float* ln_stats, int Bv, int T, int N, int H, void* stream) {
+  return opb::attention_temporal_fwd(qkv, out, ln_stats, Bv, T, N, H, static_cast<cudaStream_t>(stream));
+}
+
 int opb_relpos_lut_build(const float* table, const int32_t* idx, float* lut, int L, int H, void* stream) {
   if (!table || !idx || !lut) return OPB_ERR_INVALID;
   return opb::relpos_lut_build(table, idx, lut, L, H, static_cast<cudaStream_t>(stream));

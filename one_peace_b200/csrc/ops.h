@@ -42,6 +42,11 @@ int attention_decomp_fwd(const void* qkv, const float* lut, int lut_len, const i
                          cudaStream_t stream);
 int relpos_decomp_proj(const void* qkv, const float* rel_pos_h, const float* rel_pos_w, const int* pos_y, const int* pos_x,
                        float q_unscale, float* rel_h, float* rel_w, int B, int S, int H, int kh, int kw, cudaStream_t stream);
+// Temporal attention of the video backbone (csrc/attention_temporal.cu): softmax over the T frames of each (clip, token, head)
+// in the frame-major rows of qkv [Bv * T * N, 3 * H * 64]; out, ln_stats as attention_fwd.
+constexpr int kTemporalMinT = 2;
+constexpr int kTemporalMaxT = 32;
+int attention_temporal_fwd(const void* qkv, void* out, float* ln_stats, int Bv, int T, int N, int H, cudaStream_t stream);
 int ln_stats_finalize(const float* partial, int parts, int rows, int dim, float eps, float* mu, float* rstd,
                       cudaStream_t stream);
 

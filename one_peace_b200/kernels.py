@@ -171,6 +171,24 @@ def attention_decomp(qkv, rp, rel_h, rel_w, key_y, key_x, B, S, H, kh, kw, out=N
     return out
 
 
+def attention_temporal(qkv, Bv, T, N, H, out=None, ln_stats=None):
+    """Softmax over the T frames of every (clip, token, head) in the frame-major rows (b * T + t) * N + n of qkv
+    (include/onepeace_b200.h): -> (out bf16 [Bv * T * N, H * 64], ln_stats fp32 [H, Bv * T * N, 2])."""
+    _need_cuda(qkv, out, ln_stats)
+    D, M = H * 64, Bv * T * N
+    assert qkv.dtype == torch.bfloat16 and qkv.shape == (M, 3 * D) and qkv.is_contiguous()
+    if out is None:
+        out = torch.empty(M, D, dtype=torch.bfloat16, device=qkv.device)
+    if ln_stats is None:
+        ln_stats = torch.empty(H, M, 2, dtype=torch.float32, device=qkv.device)
+    assert out.dtype == torch.bfloat16 and out.shape == (M, D) and out.is_contiguous()
+    assert ln_stats.dtype == torch.float32 and ln_stats.numel() == H * M * 2 and ln_stats.is_contiguous()
+    st = _lib.load().opb_attention_temporal_fwd(qkv.data_ptr(), out.data_ptr(), ln_stats.data_ptr(), Bv, T, N, H, _stream())
+    _lib.check(st, "opb_attention_temporal_fwd")
+    _count()
+    return out, ln_stats
+
+
 def gemm_ln(a, w, epi, out, *, ln_mu=None, ln_rstd=None, ln_colsum=None, bias=None, colscale=None, gamma=None,
             resid=None, stats_out=None, out_bf16=None, cta_group=0, workspace=None, ln_partial=None, out_group=0,
             out_group_stride=0, out_row_offset=0, out_group_valid=0, resid_period=0, resid_row_offset=0):
