@@ -12,7 +12,8 @@ import torch.nn.functional as F
 
 from .. import kernels as K
 from .. import relpos
-from ..components import Embedding, LayerNorm, PackCache, bf16, f32, trunc_normal_
+from ..autograd import ImageEmbedFn, RelPosBiasFn, TrainBias, image_stem, pack_image_stem
+from ..components import Embedding, LayerNorm, PackCache, f32, trunc_normal_
 
 
 def make_image_bucket_position(bucket_size, num_relative_distance):
@@ -68,6 +69,29 @@ class LayerNorm2D(torch.nn.Module):
         self.layer_norm = LayerNorm(embed_dim)
 
 
+def hmlp_stem(embed_dim):
+    """`embed_images` of models/adapter/image.py:66-75: conv 4x4/4, LayerNorm2D, GELU, conv 2x2/2, LayerNorm2D, GELU,
+    conv 2x2/2, with embed_dim / 4 channels between the convs.  autograd.image_stem runs it."""
+    c4 = embed_dim // 4
+    return torch.nn.Sequential(
+        torch.nn.Conv2d(3, c4, kernel_size=4, stride=4), LayerNorm2D(c4), torch.nn.GELU(),
+        torch.nn.Conv2d(c4, c4, kernel_size=2, stride=2), LayerNorm2D(c4), torch.nn.GELU(),
+        torch.nn.Conv2d(c4, embed_dim, kernel_size=2, stride=2))
+
+
+def hmlp_stem_tensors(e):
+    """The 10 parameters of an hmlp_stem `e` in the order of autograd.pack_image_stem and ImageEmbedFn.apply."""
+    return [e[0].weight, e[0].bias, e[1].layer_norm.weight, e[1].layer_norm.bias, e[3].weight, e[3].bias,
+            e[4].layer_norm.weight, e[4].layer_norm.bias, e[6].weight, e[6].bias]
+
+
+def image_lut_bias(cache, table, bucket, side):
+    """One relative-position table over a side x side image grid plus its CLS row (S = side^2 + 1 rows) as a
+    kernels.RelPosBias in LUT form; `cache` is the caller's relpos.LutCache of its `bucket`."""
+    lut = cache.get(side * side + 1, bucket.device, bucket, lambda n: relpos.image_codes(n, side))
+    return K.RelPosBias(lut=K.relpos_lut_build(f32(table), lut[0]), code_row=lut[1], code_col=lut[2])
+
+
 class ImageAdapter(torch.nn.Module):
     def __init__(self, cfg, embed_dim, attention_heads, num_layers=None):
         super().__init__()
@@ -77,11 +101,7 @@ class ImageAdapter(torch.nn.Module):
             raise NotImplementedError("layernorm_embedding / add_type_embedding / shrink_alpha are off in the 4B config")
         self.attention_heads = attention_heads
         self.embed_dim = embed_dim
-        c4 = embed_dim // 4
-        self.embed_images = None if cfg.vision_encoder_type == "none" else torch.nn.Sequential(
-            torch.nn.Conv2d(3, c4, kernel_size=4, stride=4), LayerNorm2D(c4), torch.nn.GELU(),
-            torch.nn.Conv2d(c4, c4, kernel_size=2, stride=2), LayerNorm2D(c4), torch.nn.GELU(),
-            torch.nn.Conv2d(c4, embed_dim, kernel_size=2, stride=2))
+        self.embed_images = None if cfg.vision_encoder_type == "none" else hmlp_stem(embed_dim)
         self.cls_embedding = torch.nn.Parameter(torch.zeros(1, 1, embed_dim))
         self.bucket_size = cfg.bucket_size
         self.pos_embed = torch.nn.Parameter(torch.zeros(self.bucket_size ** 2 + 1, embed_dim))
@@ -100,23 +120,14 @@ class ImageAdapter(torch.nn.Module):
         self._pos_cache = {}
 
     def _pack(self):
-        e = self.embed_images
-        ps = [e[0].weight, e[0].bias, e[1].layer_norm.weight, e[1].layer_norm.bias, e[3].weight, e[3].bias,
-              e[4].layer_norm.weight, e[4].layer_norm.bias, e[6].weight, e[6].bias, self.cls_embedding, self.pos_embed] + \
-             ([t.weight for t in self.rel_pos_table_list] if self.rel_pos_table_list is not None else [])
+        stem = hmlp_stem_tensors(self.embed_images)
+        ps = stem + [self.cls_embedding, self.pos_embed] + \
+            ([t.weight for t in self.rel_pos_table_list] if self.rel_pos_table_list is not None else [])
 
         def build():
             self._pos_cache = {}
-            c4 = e[0].weight.shape[0]
-            return dict(
-                w1=bf16(e[0].weight.reshape(c4, 48)), b1=f32(e[0].bias),
-                ln1_w=f32(e[1].layer_norm.weight), ln1_b=f32(e[1].layer_norm.bias),
-                # conv weight [out, c, ky, kx] -> [out, (ky, kx, c)] to match the pixel-merge scatter order
-                w2=bf16(e[3].weight.permute(0, 2, 3, 1).reshape(c4, 4 * c4)), b2=f32(e[3].bias),
-                ln2_w=f32(e[4].layer_norm.weight), ln2_b=f32(e[4].layer_norm.bias),
-                w3=bf16(e[6].weight.permute(0, 2, 3, 1).reshape(self.embed_dim, 4 * c4)), b3=f32(e[6].bias),
-                cls=f32(self.cls_embedding).view(-1),
-                tables=[f32(t.weight) for t in self.rel_pos_table_list] if self.rel_pos_table_list is not None else None)
+            return dict(pack_image_stem(*stem), cls=f32(self.cls_embedding).view(-1),
+                        tables=[f32(t.weight) for t in self.rel_pos_table_list] if self.rel_pos_table_list is not None else None)
         return self._cache.get(ps, build)
 
     def get_embed_positions(self, window_size):
@@ -187,28 +198,11 @@ class ImageAdapter(torch.nn.Module):
         if torch.is_grad_enabled() and any(q.requires_grad for q in self.parameters()):
             return self.forward_train(src_images)
         p = self._pack()
-        B, _, R, _ = src_images.shape
-        d, c4 = self.embed_dim, self.embed_dim // 4
-        g1, g2, w = R // 4, R // 8, R // 16
+        w = src_images.shape[-1] // 16
         S = w * w + 1
         if self.rel_pos_table_list is not None and S != self.rp_bucket.shape[0]:
             raise RuntimeError("image size must match rel_bucket_size * 16 (one_peace_retrieval.py:128)")
-        dev = src_images.device
-        img = src_images if src_images.dtype in (torch.float32, torch.bfloat16) else src_images.float()
-        a1 = K.image_patchify4(img.contiguous())
-        y1 = torch.empty(B * g1 * g1, c4, dtype=torch.bfloat16, device=dev)
-        K.gemm(a1, p["w1"], K.EPI_STORE_BF16, y1, bias=p["b1"])
-        a2 = torch.empty(B * g2 * g2, 4 * c4, dtype=torch.bfloat16, device=dev)
-        K.layernorm(y1, p["ln1_w"], p["ln1_b"], a2, gelu=True, merge_grid_w=g1)
-        y2 = torch.empty(B * g2 * g2, c4, dtype=torch.bfloat16, device=dev)
-        K.gemm(a2, p["w2"], K.EPI_STORE_BF16, y2, bias=p["b2"])
-        a3 = torch.empty(B * w * w, 4 * c4, dtype=torch.bfloat16, device=dev)
-        K.layernorm(y2, p["ln2_w"], p["ln2_b"], a3, gelu=True, merge_grid_w=g2)
-        pos = self.get_embed_positions(w)
-        x = torch.empty(B, S, d, dtype=torch.float32, device=dev)
-        K.gemm(a3, p["w3"], K.EPI_RESID_F32, x.view(B * S, d), bias=p["b3"], resid=pos, out_group=w * w,
-               out_group_stride=S, out_row_offset=1, resid_period=w * w, resid_row_offset=1)
-        K.cls_row_init(p["cls"], pos, x)
+        x, _ = image_stem(p, src_images, self.get_embed_positions(w), p["cls"])
         bias = self.get_rel_pos_bias(S) if self.rel_pos_table_list is not None else None
         return x, None, bias
 
@@ -249,7 +243,6 @@ class ImageAdapter(torch.nn.Module):
     def forward_train(self, src_images):
         """Same outputs, recorded for autograd (autograd.ImageEmbedFn / RelPosBiasFn); the positional table is resized
         by torch ops so its gradient reaches pos_embed through torch's own bicubic adjoint (parameter preprocessing)."""
-        from ..autograd import ImageEmbedFn, RelPosBiasFn, TrainBias
         R = src_images.shape[-1]
         w = R // 16
         S = w * w + 1
@@ -261,10 +254,7 @@ class ImageAdapter(torch.nn.Module):
             # matrix (torch's bicubic kernels run single-CTA here: 2.9 ms forward + 0.9 ms backward per step)
             new = (self._resize_matrix(w, pe.device) @ pe[1:].float()).type_as(pe)
             pe = torch.cat([pe[:1], new], dim=0)
-        e = self.embed_images
-        x = ImageEmbedFn.apply(src_images, pe, e[0].weight, e[0].bias, e[1].layer_norm.weight, e[1].layer_norm.bias,
-                               e[3].weight, e[3].bias, e[4].layer_norm.weight, e[4].layer_norm.bias, e[6].weight, e[6].bias,
-                               self.cls_embedding)
+        x = ImageEmbedFn.apply(src_images, pe, *hmlp_stem_tensors(self.embed_images), self.cls_embedding)
         bias = None
         if self.rel_pos_table_list is not None:
             fast = self.get_rel_pos_bias(S)            # LUT form for the attention kernel (S <= 384), same values

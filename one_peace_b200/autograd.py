@@ -518,33 +518,58 @@ class TextEmbedFn(torch.autograd.Function):
         return None, dtable.to(tdt), dpos.to(pdt), dcls.view(cshape).to(cdt), None
 
 
+def pack_image_stem(w1, b1, ln1w, ln1b, w2, b2, ln2w, ln2b, w3, b3):
+    """The hMLP stem's parameters (convs [out, c, ky, kx], LayerNorm2D affines) as image_stem reads them: each conv weight
+    as a bf16 GEMM weight [out, (ky, kx, c)], the column order in which the LayerNorm kernel's pixel-merge scatter writes
+    that GEMM's operand; biases and affines fp32."""
+    c4, d = w1.shape[0], w3.shape[0]
+    return dict(w1=bf16(w1.reshape(c4, 48)), b1=f32(b1), ln1w=f32(ln1w), ln1b=f32(ln1b),
+                w2=bf16(w2.permute(0, 2, 3, 1).reshape(c4, 4 * c4)), b2=f32(b2), ln2w=f32(ln2w), ln2b=f32(ln2b),
+                w3=bf16(w3.permute(0, 2, 3, 1).reshape(d, 4 * c4)), b3=f32(b3))
+
+
+def image_stem(pk, img, pos, cls=None):
+    """hMLP stem (adapter/image.py:66-75) of images [B, 3, R, R] with the pack `pk` of pack_image_stem: patchify, then three
+    patch GEMMs with LayerNorm + GELU between them, the last GEMM adding the fp32 positional rows `pos`.
+    With `cls` (fp32 [d]): x fp32 [B, w*w+1, d], row 0 = cls + pos[0], row 1 + p = patch p + pos[1 + p].
+    Without: x fp32 [B*w*w, d], row-major patches, patch p + pos[p] (pos [w*w, d]).
+    Returns (x, (im, y1, a2, y2, a3)): im is the image as the patchify read it (fp32 or bf16), the rest the stages'
+    bf16 outputs, which ImageEmbedFn's backward reads."""
+    B, _, R, _ = img.shape
+    c4, d = pk["w1"].shape[0], pk["w3"].shape[0]
+    g1, g2, w = R // 4, R // 8, R // 16
+    dev = img.device
+    im = img if img.dtype in (torch.float32, torch.bfloat16) else img.float()
+    a1 = K.image_patchify4(im.contiguous())
+    y1 = K.gemm(a1, pk["w1"], K.EPI_STORE_BF16, torch.empty(B * g1 * g1, c4, dtype=torch.bfloat16, device=dev), bias=pk["b1"])
+    a2 = K.layernorm(y1, pk["ln1w"], pk["ln1b"], torch.empty(B * g2 * g2, 4 * c4, dtype=torch.bfloat16, device=dev),
+                     gelu=True, merge_grid_w=g1)
+    y2 = K.gemm(a2, pk["w2"], K.EPI_STORE_BF16, torch.empty(B * g2 * g2, c4, dtype=torch.bfloat16, device=dev), bias=pk["b2"])
+    a3 = K.layernorm(y2, pk["ln2w"], pk["ln2b"], torch.empty(B * w * w, 4 * c4, dtype=torch.bfloat16, device=dev),
+                     gelu=True, merge_grid_w=g2)
+    if cls is None:
+        x = K.gemm(a3, pk["w3"], K.EPI_RESID_F32, torch.empty(B * w * w, d, dtype=torch.float32, device=dev),
+                   bias=pk["b3"], resid=pos, resid_period=w * w)
+    else:
+        S = w * w + 1
+        x = torch.empty(B, S, d, dtype=torch.float32, device=dev)
+        K.gemm(a3, pk["w3"], K.EPI_RESID_F32, x.view(B * S, d), bias=pk["b3"], resid=pos, out_group=w * w,
+               out_group_stride=S, out_row_offset=1, resid_period=w * w, resid_row_offset=1)
+        K.cls_row_init(cls, pos, x)
+    return x, (im, y1, a2, y2, a3)
+
+
 class ImageEmbedFn(torch.autograd.Function):
-    """hMLP stem + CLS + positions (adapter/image.py:66-75,239-253) as three patch GEMMs; `pos` [S, d] is the
-    (possibly bicubic-resized, by torch autograd) positional table."""
+    """hMLP stem + CLS + positions (adapter/image.py:66-75,239-253) as three patch GEMMs (image_stem); `pos` [S, d] is
+    the (possibly bicubic-resized, by torch autograd) positional table."""
 
     @staticmethod
     def forward(ctx, img, pos, w1, b1, ln1w, ln1b, w2, b2, ln2w, ln2b, w3, b3, cls):
         B, _, R, _ = img.shape
         d = w3.shape[0]
         c4 = w1.shape[0]
-        g1, g2, w = R // 4, R // 8, R // 16
-        S = w * w + 1
-        dev = img.device
-        pk = dict(w1=bf16(w1.reshape(c4, 48)), w2=bf16(w2.permute(0, 2, 3, 1).reshape(c4, 4 * c4)),
-                  w3=bf16(w3.permute(0, 2, 3, 1).reshape(d, 4 * c4)))
-        im = img if img.dtype in (torch.float32, torch.bfloat16) else img.float()
-        a1 = K.image_patchify4(im.contiguous())
-        y1 = K.gemm(a1, pk["w1"], K.EPI_STORE_BF16, torch.empty(B * g1 * g1, c4, dtype=torch.bfloat16, device=dev), bias=f32(b1))
-        a2 = K.layernorm(y1, f32(ln1w), f32(ln1b), torch.empty(B * g2 * g2, 4 * c4, dtype=torch.bfloat16, device=dev),
-                         gelu=True, merge_grid_w=g1)
-        y2 = K.gemm(a2, pk["w2"], K.EPI_STORE_BF16, torch.empty(B * g2 * g2, c4, dtype=torch.bfloat16, device=dev), bias=f32(b2))
-        a3 = K.layernorm(y2, f32(ln2w), f32(ln2b), torch.empty(B * w * w, 4 * c4, dtype=torch.bfloat16, device=dev),
-                         gelu=True, merge_grid_w=g2)
-        posf = f32(pos)
-        x = torch.empty(B, S, d, dtype=torch.float32, device=dev)
-        K.gemm(a3, pk["w3"], K.EPI_RESID_F32, x.view(B * S, d), bias=f32(b3), resid=posf, out_group=w * w,
-               out_group_stride=S, out_row_offset=1, resid_period=w * w, resid_row_offset=1)
-        K.cls_row_init(f32(cls).view(-1), posf, x)
+        pk = pack_image_stem(w1, b1, ln1w, ln1b, w2, b2, ln2w, ln2b, w3, b3)
+        x, (im, y1, a2, y2, a3) = image_stem(pk, img, f32(pos), f32(cls).view(-1))
         ctx.save_for_backward(im, ln1w, ln1b, ln2w, ln2b, w1, w2, w3, y1, a2, y2, a3)
         ctx.pk = pk
         ctx.meta = (B, R, d, c4, pos.dtype, b1.dtype, cls.shape, cls.dtype)

@@ -27,8 +27,10 @@ import torch.nn.functional as F
 
 from .. import kernels as K
 from .. import relpos
-from ..adapter.image import LayerNorm2D, make_image_bucket_position
-from ..components import Embedding, PackCache, bf16, f32
+from . import _get_rank, resize_abs_pos_embed
+from ..adapter.image import hmlp_stem, hmlp_stem_tensors, make_image_bucket_position
+from ..autograd import image_stem, pack_image_stem
+from ..components import Embedding, PackCache, f32
 from ..transformer.multihead_attention import MultiheadAttention
 from ..transformer.transformer_encoder import TransformerEncoder
 from ..transformer.transformer_layer import TransformerEncoderLayer
@@ -58,12 +60,6 @@ except Exception:
 __all__ = ["OnePeace", "get_onepeace_lr_decay_rate"]
 
 Q_UNSCALE = 8.0      # the QKV epilogue stores q * head_dim^-0.5; the decomposed terms use the unscaled q
-
-
-def _get_rank():
-    if torch.distributed.is_available() and torch.distributed.is_initialized():
-        return torch.distributed.get_rank()
-    return 0
 
 
 def resize_table(table, src_side, dst_side):
@@ -135,11 +131,7 @@ class DetImageAdaptor(nn.Module):
                  shared_rp_bias=True, window_size=0):
         super().__init__()
         self.dropout = nn.Dropout(dropout)
-        c4 = embed_dim // 4
-        self.embed_images = nn.Sequential(
-            nn.Conv2d(3, c4, kernel_size=4, stride=4), LayerNorm2D(c4), nn.GELU(),
-            nn.Conv2d(c4, c4, kernel_size=2, stride=2), LayerNorm2D(c4), nn.GELU(),
-            nn.Conv2d(c4, embed_dim, kernel_size=2, stride=2))
+        self.embed_images = hmlp_stem(embed_dim)
         scale = embed_dim ** -0.5
         self.pretrain_bucket_size = pretrain_bucket_size
         self.bucket_size = bucket_size
@@ -157,39 +149,12 @@ class DetImageAdaptor(nn.Module):
         self._lut_cache = PackCache()
         self._layout = {}
 
-    def _stem_pack(self):
-        e = self.embed_images
-        ps = [e[0].weight, e[0].bias, e[1].layer_norm.weight, e[1].layer_norm.bias, e[3].weight, e[3].bias,
-              e[4].layer_norm.weight, e[4].layer_norm.bias, e[6].weight, e[6].bias, self.pos_embed]
-
-        def build():
-            w1, b1, l1w, l1b, w2, b2, l2w, l2b, w3, b3, pos = ps
-            c4, d = w1.shape[0], w3.shape[0]
-            return dict(w1=bf16(w1.reshape(c4, 48)), b1=f32(b1), l1w=f32(l1w), l1b=f32(l1b),
-                        w2=bf16(w2.permute(0, 2, 3, 1).reshape(c4, 4 * c4)), b2=f32(b2), l2w=f32(l2w), l2b=f32(l2b),
-                        w3=bf16(w3.permute(0, 2, 3, 1).reshape(d, 4 * c4)), b3=f32(b3),
-                        pos=f32(pos[1:]).contiguous())
-        return self._stem_cache.get(ps, build)
-
     def stem(self, img):
         """hMLP stem + pos_embed[1:] (onepeace.py:146-152) -> fp32 [B * side^2, d], row-major grid per sample."""
-        pk = self._stem_pack()
-        B, _, R, _ = img.shape
-        c4, d = pk["w1"].shape[0], pk["w3"].shape[0]
-        g1, g2, w = R // 4, R // 8, R // 16
-        dev = img.device
-        im = img if img.dtype in (torch.float32, torch.bfloat16) else img.float()
-        a1 = K.image_patchify4(im.contiguous())
-        y1 = K.gemm(a1, pk["w1"], K.EPI_STORE_BF16, torch.empty(B * g1 * g1, c4, dtype=torch.bfloat16, device=dev),
-                    bias=pk["b1"])
-        a2 = K.layernorm(y1, pk["l1w"], pk["l1b"], torch.empty(B * g2 * g2, 4 * c4, dtype=torch.bfloat16, device=dev),
-                         gelu=True, merge_grid_w=g1)
-        y2 = K.gemm(a2, pk["w2"], K.EPI_STORE_BF16, torch.empty(B * g2 * g2, c4, dtype=torch.bfloat16, device=dev),
-                    bias=pk["b2"])
-        a3 = K.layernorm(y2, pk["l2w"], pk["l2b"], torch.empty(B * w * w, 4 * c4, dtype=torch.bfloat16, device=dev),
-                         gelu=True, merge_grid_w=g2)
-        x = torch.empty(B * w * w, d, dtype=torch.float32, device=dev)
-        return K.gemm(a3, pk["w3"], K.EPI_RESID_F32, x, bias=pk["b3"], resid=pk["pos"], resid_period=w * w)
+        stem = hmlp_stem_tensors(self.embed_images)
+        pk = self._stem_cache.get(stem + [self.pos_embed],
+                                  lambda: dict(pack_image_stem(*stem), pos=f32(self.pos_embed[1:])))
+        return image_stem(pk, img, pk["pos"])[0]
 
     def luts(self):
         """(global, window) LUT-form biases of the shared table, resized as get_rel_pos_bias (onepeace.py:123-144) does;
@@ -293,19 +258,7 @@ class OnePeace(Backbone):
                 print(self.load_state_dict(checkpoint_model, strict=False))
                 print(f"Loading OFA Encoder pretrained weights from {pretrained}.")
 
-    def resize_abs_pos_embed(self, checkpoint):
-        """onepeace.py:535-558: bicubic resize of the checkpoint's positional rows, the first row kept."""
-        pos = checkpoint["image_adapter.pos_embed"]
-        dim = pos.shape[-1]
-        num_patches = self.image_adapter.bucket_size ** 2
-        extra = self.image_adapter.pos_embed.shape[-2] - num_patches
-        orig, new = int((pos.shape[-2] - extra) ** 0.5), int(num_patches ** 0.5)
-        if orig != new:
-            if _get_rank() == 0:
-                print(f"Position interpolate from {orig}x{orig} to {new}x{new}")
-            tok = pos[extra:].reshape(-1, orig, orig, dim).permute(0, 3, 1, 2)
-            tok = F.interpolate(tok, size=(new, new), mode="bicubic", align_corners=False)
-            checkpoint["image_adapter.pos_embed"] = torch.cat((pos[:extra], tok.permute(0, 2, 3, 1).flatten(0, 2)), dim=0)
+    resize_abs_pos_embed = resize_abs_pos_embed
 
     def resize_rel_pos_embed(self, checkpoint):
         """onepeace.py:560-613 with shared_rp_bias=True: rel_pos_table_list.0.weight -> rel_pos_table.weight, rp_bucket keys

@@ -25,7 +25,7 @@ import torch.nn as nn
 
 from .. import kernels as K
 from .. import relpos
-from ..adapter.image import LayerNorm2D, make_image_bucket_position
+from ..adapter.image import hmlp_stem, hmlp_stem_tensors, image_lut_bias, make_image_bucket_position
 from ..autograd import ImageEmbedFn, RelPosBiasFn, TrainBias, _pad8, run_encoder_stack
 from ..autograd_classify import VitHeadFn
 from ..components import Embedding, PackCache, bf16, f32
@@ -42,11 +42,7 @@ class ImageAdaptor(nn.Module):
 
     def __init__(self, attention_heads, bucket_size, embed_dim):
         super().__init__()
-        c4 = embed_dim // 4
-        self.embed_images = nn.Sequential(
-            nn.Conv2d(3, c4, kernel_size=4, stride=4), LayerNorm2D(c4), nn.GELU(),
-            nn.Conv2d(c4, c4, kernel_size=2, stride=2), LayerNorm2D(c4), nn.GELU(),
-            nn.Conv2d(c4, embed_dim, kernel_size=2, stride=2))
+        self.embed_images = hmlp_stem(embed_dim)
         scale = embed_dim ** -0.5
         self.cls_embedding = nn.Parameter(scale * torch.randn(1, 1, embed_dim))
         self.bucket_size = bucket_size
@@ -64,17 +60,11 @@ class ImageAdaptor(nn.Module):
         if src_images.dim() != 4 or src_images.shape[-2] != R or R != 16 * self.bucket_size:
             raise ValueError(f"OnePeaceViT with bucket_size {self.bucket_size} takes [B, 3, {16 * self.bucket_size}, "
                              f"{16 * self.bucket_size}] images, got {tuple(src_images.shape)}")
-        e = self.embed_images
-        x = ImageEmbedFn.apply(src_images, self.pos_embed, e[0].weight, e[0].bias, e[1].layer_norm.weight,
-                               e[1].layer_norm.bias, e[3].weight, e[3].bias, e[4].layer_norm.weight, e[4].layer_norm.bias,
-                               e[6].weight, e[6].bias, self.cls_embedding)
+        x = ImageEmbedFn.apply(src_images, self.pos_embed, *hmlp_stem_tensors(self.embed_images), self.cls_embedding)
         S = self.bucket_size ** 2 + 1
         H = self.attention_heads
         table = self.rel_pos_table.weight
-        lut = self._lut_cache.get(S, self.rp_bucket.device, self.rp_bucket, lambda n: relpos.image_codes(n, self.bucket_size)) \
-            if S <= K.ATTN_TC_MAX_S else None
-        fast = K.RelPosBias(lut=K.relpos_lut_build(f32(table), lut[0]), code_row=lut[1], code_col=lut[2]) \
-            if lut is not None else None
+        fast = image_lut_bias(self._lut_cache, table, self.rp_bucket, self.bucket_size) if S <= K.ATTN_TC_MAX_S else None
         if train:
             return x, [TrainBias(RelPosBiasFn.apply(table, self.rp_bucket, S, H), fast)]
         if fast is None:

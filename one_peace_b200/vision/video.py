@@ -24,11 +24,12 @@ import pickle
 
 import torch
 import torch.nn as nn
-import torch.nn.functional as F
 
 from .. import kernels as K
 from .. import relpos
-from ..adapter.image import LayerNorm2D, geometric_sequence_interpolation, make_image_bucket_position
+from . import _get_rank, resize_abs_pos_embed
+from ..adapter.image import (geometric_sequence_interpolation, hmlp_stem, hmlp_stem_tensors, image_lut_bias,
+                             make_image_bucket_position)
 from ..autograd import ImageEmbedFn
 from ..components import Embedding, PackCache, bf16, f32
 from ..transformer.transformer_layer import TransformerEncoderLayer
@@ -42,12 +43,6 @@ except Exception:
         return cls
 
 __all__ = ["OnePeaceViT"]
-
-
-def _get_rank():
-    if torch.distributed.is_available() and torch.distributed.is_initialized():
-        return torch.distributed.get_rank()
-    return 0
 
 
 class Adapter(nn.Module):
@@ -70,11 +65,7 @@ class ImageAdaptor(nn.Module):
                  shared_rp_bias=True):
         super().__init__()
         self.dropout_module = nn.Dropout(dropout)
-        c4 = embed_dim // 4
-        self.embed_images = nn.Sequential(
-            nn.Conv2d(3, c4, kernel_size=4, stride=4), LayerNorm2D(c4), nn.GELU(),
-            nn.Conv2d(c4, c4, kernel_size=2, stride=2), LayerNorm2D(c4), nn.GELU(),
-            nn.Conv2d(c4, embed_dim, kernel_size=2, stride=2))
+        self.embed_images = hmlp_stem(embed_dim)
         scale = embed_dim ** -0.5
         self.cls_embedding = nn.Parameter(scale * torch.randn(1, 1, embed_dim))
         self.bucket_size = bucket_size
@@ -91,10 +82,7 @@ class ImageAdaptor(nn.Module):
     def stem(self, frames):
         """hMLP stem + CLS + pos_embed + temporal_embedding (onepeace.py:187-201) of frames [B T, 3, R, R], clip-major
         -> fp32 [B T N, d] frame-major rows."""
-        e = self.embed_images
-        x = ImageEmbedFn.apply(frames, self.pos_embed, e[0].weight, e[0].bias, e[1].layer_norm.weight,
-                               e[1].layer_norm.bias, e[3].weight, e[3].bias, e[4].layer_norm.weight, e[4].layer_norm.bias,
-                               e[6].weight, e[6].bias, self.cls_embedding)
+        x = ImageEmbedFn.apply(frames, self.pos_embed, *hmlp_stem_tensors(self.embed_images), self.cls_embedding)
         BT, N, d = x.shape
         T = self.num_frames
         add = self._temporal_cache.get([self.temporal_embedding],
@@ -109,10 +97,7 @@ class ImageAdaptor(nn.Module):
         if S > K.ATTN_TC_MAX_S:
             raise NotImplementedError(f"OnePeaceViT: bucket_size {self.bucket_size} gives {S} tokens per frame; the LUT-form "
                                       f"attention is built for at most {K.ATTN_TC_MAX_S}")
-        lut = self._lut_cache.get(S, self.rp_bucket.device, self.rp_bucket,
-                                  lambda n: relpos.image_codes(n, self.bucket_size))
-        return K.RelPosBias(lut=K.relpos_lut_build(f32(self.rel_pos_table.weight), lut[0]), code_row=lut[1],
-                            code_col=lut[2])
+        return image_lut_bias(self._lut_cache, self.rel_pos_table.weight, self.rp_bucket, self.bucket_size)
 
 
 class VideoLayer(TransformerEncoderLayer):
@@ -247,19 +232,7 @@ class OnePeaceViT(nn.Module):
         self.shared_rp_bias = shared_rp_bias
         self.use_checkpoint = use_checkpoint
 
-    def resize_abs_pos_embed(self, checkpoint):
-        """onepeace.py:526-551: bicubic resize of the checkpoint's positional rows, the first row kept."""
-        pos = checkpoint["image_adapter.pos_embed"]
-        dim = pos.shape[-1]
-        num_patches = self.image_adapter.bucket_size ** 2
-        extra = self.image_adapter.pos_embed.shape[-2] - num_patches
-        orig, new = int((pos.shape[-2] - extra) ** 0.5), int(num_patches ** 0.5)
-        if orig != new:
-            if _get_rank() == 0:
-                print("Position interpolate from %dx%d to %dx%d" % (orig, orig, new, new))
-            tok = pos[extra:].reshape(-1, orig, orig, dim).permute(0, 3, 1, 2)
-            tok = F.interpolate(tok, size=(new, new), mode="bicubic", align_corners=False)
-            checkpoint["image_adapter.pos_embed"] = torch.cat((pos[:extra], tok.permute(0, 2, 3, 1).flatten(0, 2)), dim=0)
+    resize_abs_pos_embed = resize_abs_pos_embed
 
     def resize_rel_pos_embed(self, checkpoint):
         """onepeace.py:553-609 with shared_rp_bias=True: rel_pos_table_list.0.weight -> rel_pos_table.weight, the
