@@ -154,6 +154,17 @@ int opb_attention_decomp_fwd(const void* qkv, const float* lut, int lut_len, con
 int opb_attention_temporal_fwd(const void* qkv, void* out, float* ln_stats, int Bv, int T, int N, int H, void* stream);
 
 /*
+ * Adjoint of opb_attention_temporal_fwd.  qkv is the forward's operand, out its output and d_out the gradient of out, all in
+ * the same frame-major rows and read in place at a stride of N rows.  Writes every element of dqkv bf16
+ * [Bv * T * N, 3 * H * 64] = [dq | dk | dv], dq multiplied by q_scale (the gradient of the un-scaled projection, as
+ * opb_attention_bwd).  P is recomputed with the forward's arithmetic, so no log-sum-exp is needed.  No atomics: repeated
+ * launches are bit-identical.  Needs 2 <= T <= 32, Bv, N, H >= 1 and non-null 16-byte aligned pointers; anything else
+ * returns OPB_ERR_INVALID before a launch.
+ */
+int opb_attention_temporal_bwd(const void* qkv, const void* out, const void* d_out, void* dqkv, int Bv, int T, int N, int H,
+                               float q_scale, void* stream);
+
+/*
  * GEMM with the full epilogue description (superset of opb_gemm_bf16).  Adds the fused-LayerNorm form
  *   LN(x) W^T + b  =  rstd[m] * (acc - mu[m] * colsum[n]) + bias'[n]
  * where A holds the UN-normalised rows (bf16), B = W * diag(ln_weight) (bf16), colsum[n] = sum_k B[n,k],
@@ -373,6 +384,11 @@ int opb_layernorm_bwd(const void* x, int x_dtype, int64_t ldx, const void* dy, i
  * its adjoint dgl = [du * l * gelu'(g) | du * gelu(g)]. */
 int opb_geglu_fwd(const void* gl, void* u, int64_t rows, int F, void* stream);
 int opb_geglu_bwd(const void* gl, const void* du, void* dgl, int64_t rows, int F, void* stream);
+
+/* Exact-erf GELU on the video adapters' bf16 pre-activations z [rows, F] (onepeace.py:29-39): y = gelu_erf(z), and its
+ * adjoint dz = dy * gelu'(z).  F % 8 == 0, 16-byte aligned non-null pointers, else OPB_ERR_INVALID. */
+int opb_gelu_fwd(const void* z, void* y, int64_t rows, int F, void* stream);
+int opb_gelu_bwd(const void* z, const void* dy, void* dz, int64_t rows, int F, void* stream);
 
 /* LayerScale + drop-path residual (transformer_layer.py:70-88): out = x + row_scale[r] * gamma[n] * o  (o bf16; gamma /
  * row_scale may be NULL = 1) and its adjoint: d_o = bf16(row_scale * gamma * dx), dgamma = sum_r row_scale * dx * o,

@@ -34,6 +34,8 @@ SIGNATURES = {
     "opb_attention_decomp_fwd": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                          c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
     "opb_attention_temporal_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
+    "opb_attention_temporal_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float,
+                                           c_void_p]),
     "opb_gemm_bf16_ex": (c_int, [c_void_p, c_void_p]),
     "opb_row_stats_cast": (c_int, [c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_void_p, c_int, c_int, c_float, c_void_p]),
     "opb_ln_stats_finalize": (c_int, [c_void_p, c_int, c_int, c_int, c_float, c_void_p, c_void_p, c_void_p]),
@@ -78,6 +80,8 @@ SIGNATURES.update({
     "opb_text_embed_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
     "opb_geglu_fwd": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_void_p]),
     "opb_geglu_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int, c_void_p]),
+    "opb_gelu_fwd": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_void_p]),
+    "opb_gelu_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int, c_void_p]),
     "opb_scale_resid_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int, c_void_p]),
     "opb_scale_resid_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int,
                                     c_int, c_int, c_int, c_int, c_void_p]),

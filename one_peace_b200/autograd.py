@@ -45,20 +45,23 @@ def _pad8(n):
     return (n + 7) // 8 * 8
 
 
-def keep_activations(n_layers, rows, d, ffn, device):
+def keep_activations(n_layers, rows, d, ffn, device, row_bytes=None):
     """Activation policy of the training stack.  The reference wraps every layer in checkpoint_wrapper (one_peace_pretrain.py
     :83-91, `checkpoint_activations` in the 4B recipes) because 12,608 rows x 40 layers of layer activations (1.05 GB per layer
     at d = 1536, ffn = 6144) do not fit an 80 GB part next to the model.  When the activations of the whole
     stack fit in half of the memory that is free right now they are KEPT and the backward skips the recompute (a quarter of
     the step's GEMM work); otherwise each layer is recomputed while its adjoint runs, as the reference does.
-    OPB_ACTIVATIONS=keep | recompute overrides the choice (tests exercise both)."""
+    OPB_ACTIVATIONS=keep | recompute overrides the choice (tests exercise both).  `row_bytes`: the saved bytes per row of
+    a layer whose activations differ from the encoder layer's (the video layer's)."""
     mode = __import__("os").environ.get("OPB_ACTIVATIONS", "auto")
     if mode in ("keep", "recompute"):
         return mode == "keep"
-    key = (n_layers, rows, d, ffn)
+    key = (n_layers, rows, d, ffn, row_bytes)
     if torch.cuda.is_current_stream_capturing():               # no driver queries under capture: reuse the warm-up's decision
         return _POLICY.get(key, False)
-    need = n_layers * rows * (22 * d + 8 * ffn + 64)          # bytes: h1 qkv att a2 o x2(fp32) h2 f | gl u u2 | lse
+    if row_bytes is None:
+        row_bytes = 22 * d + 8 * ffn + 64                      # bytes: h1 qkv att a2 o x2(fp32) h2 f | gl u u2 | lse
+    need = n_layers * rows * row_bytes
     free, _ = torch.cuda.mem_get_info(device)
     _POLICY[key] = need < free // 2
     return _POLICY[key]

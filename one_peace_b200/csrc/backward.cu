@@ -2,6 +2,7 @@
 // transformer_layer.py:165-228, multihead_attention.py:103-126, components.py:23-44):
 //   layernorm_bwd     dx, dgamma, dbeta of  y = LN(x) * gamma + beta  (optionally y = gelu(LN(x)...), the hMLP stem)
 //   geglu_fwd/bwd     u = gelu_erf(g) * l  on the un-fused [M, 2F] projection (transformer_layer.py:54-67)
+//   gelu_fwd/bwd      y = gelu_erf(z) on the video adapters' [M, F] pre-activations (onepeace.py:29-39) and dz = dy gelu'(z)
 //   scale_resid_fwd   x_out = x + row_scale * gamma * o           (LayerScale + drop-path residual, :70-88)
 //   scale_resid_bwd   do = row_scale * gamma * dx, dgamma = sum_rows row_scale * dx * o, dbias = sum_rows do
 //   colsum            bias gradients: sum over rows of a bf16 [M, n] matrix
@@ -342,6 +343,30 @@ geglu_bwd_kernel(const __nv_bfloat16* __restrict__ gl, const __nv_bfloat16* __re
   }
 }
 
+__global__ void __launch_bounds__(256)
+gelu_fwd_kernel(const __nv_bfloat16* __restrict__ z, __nv_bfloat16* __restrict__ y, long n8) {
+  for (long i = static_cast<long>(blockIdx.x) * 256 + threadIdx.x; i < n8; i += static_cast<long>(gridDim.x) * 256) {
+    float f[8];
+    unpack8(reinterpret_cast<const uint4*>(z)[i], f);
+#pragma unroll
+    for (int e = 0; e < 8; ++e) f[e] = gelu_erf(f[e]);
+    reinterpret_cast<uint4*>(y)[i] = pack8(f);
+  }
+}
+
+__global__ void __launch_bounds__(256)
+gelu_bwd_kernel(const __nv_bfloat16* __restrict__ z, const __nv_bfloat16* __restrict__ dy, __nv_bfloat16* __restrict__ dz,
+                long n8) {
+  for (long i = static_cast<long>(blockIdx.x) * 256 + threadIdx.x; i < n8; i += static_cast<long>(gridDim.x) * 256) {
+    float f[8], d[8];
+    unpack8(reinterpret_cast<const uint4*>(z)[i], f);
+    unpack8(reinterpret_cast<const uint4*>(dy)[i], d);
+#pragma unroll
+    for (int e = 0; e < 8; ++e) f[e] = d[e] * gelu_grad(f[e]);
+    reinterpret_cast<uint4*>(dz)[i] = pack8(f);
+  }
+}
+
 // ---------------------------------------------------------------------------------------------------------------
 __global__ void scale_resid_fwd_kernel(const float* __restrict__ x, const __nv_bfloat16* __restrict__ o,
                                        const float* __restrict__ gamma, const float* __restrict__ row_scale,
@@ -640,6 +665,26 @@ int geglu_bwd(const void* gl, const void* du, void* dgl, long rows, int F, cudaS
   geglu_bwd_kernel<<<dim3(gx, gy > 0 ? gy : 1), 256, 0, stream>>>(
       reinterpret_cast<const __nv_bfloat16*>(gl), reinterpret_cast<const __nv_bfloat16*>(du),
       reinterpret_cast<__nv_bfloat16*>(dgl), rows, F);
+  return cudaGetLastError() == cudaSuccess ? OPB_OK : OPB_ERR_CUDA;
+}
+
+int gelu_fwd(const void* z, void* y, long rows, int F, cudaStream_t stream) {
+  if (rows <= 0 || F <= 0 || (F & 7) || ((reinterpret_cast<uintptr_t>(z) | reinterpret_cast<uintptr_t>(y)) & 15))
+    return OPB_ERR_INVALID;
+  const long n8 = rows * (F / 8);
+  gelu_fwd_kernel<<<elementwise_grid(n8), 256, 0, stream>>>(reinterpret_cast<const __nv_bfloat16*>(z),
+                                                             reinterpret_cast<__nv_bfloat16*>(y), n8);
+  return cudaGetLastError() == cudaSuccess ? OPB_OK : OPB_ERR_CUDA;
+}
+
+int gelu_bwd(const void* z, const void* dy, void* dz, long rows, int F, cudaStream_t stream) {
+  if (rows <= 0 || F <= 0 || (F & 7) ||
+      ((reinterpret_cast<uintptr_t>(z) | reinterpret_cast<uintptr_t>(dy) | reinterpret_cast<uintptr_t>(dz)) & 15))
+    return OPB_ERR_INVALID;
+  const long n8 = rows * (F / 8);
+  gelu_bwd_kernel<<<elementwise_grid(n8), 256, 0, stream>>>(reinterpret_cast<const __nv_bfloat16*>(z),
+                                                             reinterpret_cast<const __nv_bfloat16*>(dy),
+                                                             reinterpret_cast<__nv_bfloat16*>(dz), n8);
   return cudaGetLastError() == cudaSuccess ? OPB_OK : OPB_ERR_CUDA;
 }
 

@@ -63,6 +63,11 @@ int opb_attention_temporal_fwd(const void* qkv, void* out, float* ln_stats, int 
   return opb::attention_temporal_fwd(qkv, out, ln_stats, Bv, T, N, H, static_cast<cudaStream_t>(stream));
 }
 
+int opb_attention_temporal_bwd(const void* qkv, const void* out, const void* d_out, void* dqkv, int Bv, int T, int N, int H,
+                               float q_scale, void* stream) {
+  return opb::attention_temporal_bwd(qkv, out, d_out, dqkv, Bv, T, N, H, q_scale, static_cast<cudaStream_t>(stream));
+}
+
 int opb_relpos_lut_build(const float* table, const int32_t* idx, float* lut, int L, int H, void* stream) {
   if (!table || !idx || !lut) return OPB_ERR_INVALID;
   return opb::relpos_lut_build(table, idx, lut, L, H, static_cast<cudaStream_t>(stream));
@@ -287,6 +292,16 @@ int opb_geglu_fwd(const void* gl, void* u, int64_t rows, int F, void* stream) {
 int opb_geglu_bwd(const void* gl, const void* du, void* dgl, int64_t rows, int F, void* stream) {
   if (!gl || !du || !dgl) return OPB_ERR_INVALID;
   return opb::geglu_bwd(gl, du, dgl, rows, F, static_cast<cudaStream_t>(stream));
+}
+
+int opb_gelu_fwd(const void* z, void* y, int64_t rows, int F, void* stream) {
+  if (!z || !y) return OPB_ERR_INVALID;
+  return opb::gelu_fwd(z, y, rows, F, static_cast<cudaStream_t>(stream));
+}
+
+int opb_gelu_bwd(const void* z, const void* dy, void* dz, int64_t rows, int F, void* stream) {
+  if (!z || !dy || !dz) return OPB_ERR_INVALID;
+  return opb::gelu_bwd(z, dy, dz, rows, F, static_cast<cudaStream_t>(stream));
 }
 
 int opb_scale_resid_fwd(const float* x, const void* o, const float* gamma, const float* row_scale, float* out,

@@ -47,6 +47,9 @@ int relpos_decomp_proj(const void* qkv, const float* rel_pos_h, const float* rel
 constexpr int kTemporalMinT = 2;
 constexpr int kTemporalMaxT = 32;
 int attention_temporal_fwd(const void* qkv, void* out, float* ln_stats, int Bv, int T, int N, int H, cudaStream_t stream);
+// its adjoint: dqkv [Bv * T * N, 3 * H * 64] from qkv, the forward output and its gradient (dq multiplied by q_scale)
+int attention_temporal_bwd(const void* qkv, const void* out, const void* d_out, void* dqkv, int Bv, int T, int N, int H,
+                           float q_scale, cudaStream_t stream);
 int ln_stats_finalize(const float* partial, int parts, int rows, int dim, float eps, float* mu, float* rstd,
                       cudaStream_t stream);
 
@@ -147,6 +150,8 @@ int layernorm_bwd(const void* x, int x_dtype, long ldx, const void* dy, int dy_d
                   int gelu, int dy_merge_w, float* ws, float* dgamma, float* dbeta, cudaStream_t stream);
 int geglu_fwd(const void* gl, void* u, long rows, int F, cudaStream_t stream);
 int geglu_bwd(const void* gl, const void* du, void* dgl, long rows, int F, cudaStream_t stream);
+int gelu_fwd(const void* z, void* y, long rows, int F, cudaStream_t stream);
+int gelu_bwd(const void* z, const void* dy, void* dz, long rows, int F, cudaStream_t stream);
 int scale_resid_fwd(const float* x, const void* o, const float* gamma, const float* row_scale, float* out, long rows,
                     int n, cudaStream_t stream);
 int scale_resid_bwd(const float* dx, const void* o, const float* gamma, const float* row_scale, void* d_o, float* ws,

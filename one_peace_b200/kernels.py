@@ -189,6 +189,24 @@ def attention_temporal(qkv, Bv, T, N, H, out=None, ln_stats=None):
     return out, ln_stats
 
 
+def attention_temporal_bwd(qkv, out, d_out, Bv, T, N, H, q_scale, dqkv=None):
+    """Adjoint of attention_temporal (include/onepeace_b200.h): -> dqkv bf16 [Bv * T * N, 3 * H * 64] in the same rows,
+    dq multiplied by q_scale."""
+    _need_cuda(qkv, out, d_out, dqkv)
+    D, M = H * 64, Bv * T * N
+    assert qkv.dtype == torch.bfloat16 and qkv.shape == (M, 3 * D) and qkv.is_contiguous()
+    for t in (out, d_out):
+        assert t.dtype == torch.bfloat16 and t.shape == (M, D) and t.is_contiguous()
+    if dqkv is None:
+        dqkv = torch.empty(M, 3 * D, dtype=torch.bfloat16, device=qkv.device)
+    assert dqkv.dtype == torch.bfloat16 and dqkv.shape == (M, 3 * D) and dqkv.is_contiguous()
+    st = _lib.load().opb_attention_temporal_bwd(qkv.data_ptr(), out.data_ptr(), d_out.data_ptr(), dqkv.data_ptr(), Bv, T, N,
+                                                H, float(q_scale), _stream())
+    _lib.check(st, "opb_attention_temporal_bwd")
+    _count()
+    return dqkv
+
+
 def gemm_ln(a, w, epi, out, *, ln_mu=None, ln_rstd=None, ln_colsum=None, bias=None, colscale=None, gamma=None,
             resid=None, stats_out=None, out_bf16=None, cta_group=0, workspace=None, ln_partial=None, out_group=0,
             out_group_stride=0, out_row_offset=0, out_group_valid=0, resid_period=0, resid_row_offset=0):
@@ -547,6 +565,26 @@ def geglu_bwd(gl, du, dgl):
     _lib.check(st, "opb_geglu_bwd")
     _count()
     return dgl
+
+
+def gelu_fwd(z, y):
+    """y = gelu_erf(z), bf16 [rows, F] (row-contiguous)"""
+    rows, F = z.shape
+    assert z.is_contiguous() and y.is_contiguous() and y.shape == z.shape
+    st = _lib.load().opb_gelu_fwd(z.data_ptr(), y.data_ptr(), rows, F, _stream())
+    _lib.check(st, "opb_gelu_fwd")
+    _count()
+    return y
+
+
+def gelu_bwd(z, dy, dz):
+    """dz = dy * gelu'(z), bf16 [rows, F]"""
+    rows, F = z.shape
+    assert z.is_contiguous() and dy.is_contiguous() and dz.is_contiguous() and dy.shape == z.shape == dz.shape
+    st = _lib.load().opb_gelu_bwd(z.data_ptr(), dy.data_ptr(), dz.data_ptr(), rows, F, _stream())
+    _lib.check(st, "opb_gelu_bwd")
+    _count()
+    return dz
 
 
 def scale_resid_fwd(x, o, gamma, row_scale, out):
