@@ -165,6 +165,34 @@ int opb_attention_temporal_bwd(const void* qkv, const void* out, const void* d_o
                                float q_scale, void* stream);
 
 /*
+ * Multi-scale deformable attention core (one_peace_vision/seg/ops, MSDeformAttn) with D = 32 channels per head, fused with
+ * the soft-max over each head's L * P logits and the sampling locations loc = ref + off / (W_l, H_l).
+ *   value : bf16 [N * S_in, H * 32], the value_proj output; level l of sample n owns rows n * S_in + start_l + y * W_l + x.
+ *   proj  : fp32 [N * Lq, 3 * H * L * P] = [offsets (h, l, p, xy) | logits (h, l * P + p)], the reference's orders.
+ *   ref   : fp32 [N * Lq, L_ref, 2] reference points (x, y), L_ref = 1 (shared by every level) or L.
+ *   level_hw [L, 2] = (H_l, W_l) and level_start [L]: HOST int32 arrays, passed to the kernel by value (no device copy).
+ *   out   : bf16 [N * Lq, H * 32] = sum over (l, p) of softmax(logits)_lp * bilinear(value_l, loc * (W_l, H_l) - 0.5), taps
+ *           outside the level read as zero (grid_sample, align_corners = False, padding_mode = zeros); fp32 accumulation.
+ * No atomics, one write per output element: repeated launches are bit-identical.  Needs D == 32, 1 <= L <= 4, 1 <= P <= 8,
+ * L_ref in {1, L}, N, S_in, Lq, H >= 1, every level inside S_in and non-null 16-byte aligned device pointers; anything else
+ * returns OPB_ERR_INVALID before a launch.
+ */
+int opb_ms_deform_attn_fwd(const void* value, const float* proj, const float* ref, void* out, int N, int S_in, int Lq, int H,
+                           int D, int L, int P, int L_ref, const int32_t* level_hw, const int32_t* level_start, void* stream);
+
+/*
+ * Adjoint of opb_ms_deform_attn_fwd for d_out bf16 [N * Lq, H * 32], with the forward's arguments.
+ *   d_value : fp32 [N * S_in, H * 32], ACCUMULATED (the caller zeroes it): a_lp * tap weight * d_out, scattered with fp32
+ *             vector atomics, so repeats differ in the last bits.
+ *   d_proj  : fp32 [N * Lq, 3 * H * L * P], every element written: the offset gradients d_loc / (W_l, H_l) (taps outside
+ *             the level contribute nothing) and the logit gradients a * (dA - sum a dA).  No atomics: bit-identical repeats.
+ * No gradient of the reference points.  Argument checks as the forward.
+ */
+int opb_ms_deform_attn_bwd(const void* value, const float* proj, const float* ref, const void* d_out, float* d_value,
+                           float* d_proj, int N, int S_in, int Lq, int H, int D, int L, int P, int L_ref,
+                           const int32_t* level_hw, const int32_t* level_start, void* stream);
+
+/*
  * GEMM with the full epilogue description (superset of opb_gemm_bf16).  Adds the fused-LayerNorm form
  *   LN(x) W^T + b  =  rstd[m] * (acc - mu[m] * colsum[n]) + bias'[n]
  * where A holds the UN-normalised rows (bf16), B = W * diag(ln_weight) (bf16), colsum[n] = sum_k B[n,k],

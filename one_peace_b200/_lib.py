@@ -36,6 +36,10 @@ SIGNATURES = {
     "opb_attention_temporal_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
     "opb_attention_temporal_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_float,
                                            c_void_p]),
+    "opb_ms_deform_attn_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int,
+                                       c_int, c_int, c_void_p, c_void_p, c_void_p]),
+    "opb_ms_deform_attn_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int,
+                                       c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     "opb_gemm_bf16_ex": (c_int, [c_void_p, c_void_p]),
     "opb_row_stats_cast": (c_int, [c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_void_p, c_int, c_int, c_float, c_void_p]),
     "opb_ln_stats_finalize": (c_int, [c_void_p, c_int, c_int, c_int, c_float, c_void_p, c_void_p, c_void_p]),

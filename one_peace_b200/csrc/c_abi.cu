@@ -68,6 +68,19 @@ int opb_attention_temporal_bwd(const void* qkv, const void* out, const void* d_o
   return opb::attention_temporal_bwd(qkv, out, d_out, dqkv, Bv, T, N, H, q_scale, static_cast<cudaStream_t>(stream));
 }
 
+int opb_ms_deform_attn_fwd(const void* value, const float* proj, const float* ref, void* out, int N, int S_in, int Lq, int H,
+                           int D, int L, int P, int L_ref, const int32_t* level_hw, const int32_t* level_start, void* stream) {
+  return opb::ms_deform_attn_fwd(value, proj, ref, out, N, S_in, Lq, H, D, L, P, L_ref, level_hw, level_start,
+                                 static_cast<cudaStream_t>(stream));
+}
+
+int opb_ms_deform_attn_bwd(const void* value, const float* proj, const float* ref, const void* d_out, float* d_value,
+                           float* d_proj, int N, int S_in, int Lq, int H, int D, int L, int P, int L_ref,
+                           const int32_t* level_hw, const int32_t* level_start, void* stream) {
+  return opb::ms_deform_attn_bwd(value, proj, ref, d_out, d_value, d_proj, N, S_in, Lq, H, D, L, P, L_ref, level_hw,
+                                 level_start, static_cast<cudaStream_t>(stream));
+}
+
 int opb_relpos_lut_build(const float* table, const int32_t* idx, float* lut, int L, int H, void* stream) {
   if (!table || !idx || !lut) return OPB_ERR_INVALID;
   return opb::relpos_lut_build(table, idx, lut, L, H, static_cast<cudaStream_t>(stream));

@@ -50,6 +50,15 @@ int attention_temporal_fwd(const void* qkv, void* out, float* ln_stats, int Bv, 
 // its adjoint: dqkv [Bv * T * N, 3 * H * 64] from qkv, the forward output and its gradient (dq multiplied by q_scale)
 int attention_temporal_bwd(const void* qkv, const void* out, const void* d_out, void* dqkv, int Bv, int T, int N, int H,
                            float q_scale, cudaStream_t stream);
+// Multi-scale deformable attention (csrc/ms_deform_attn.cu), D = 32 channels per head; level_hw [L, 2] (H_l, W_l) and
+// level_start [L] are host arrays, passed to the kernel by value.
+constexpr int kMsdaMaxL = 4;
+constexpr int kMsdaMaxP = 8;
+int ms_deform_attn_fwd(const void* value, const float* proj, const float* ref, void* out, int N, int S_in, int Lq, int H,
+                       int D, int L, int P, int L_ref, const int* level_hw, const int* level_start, cudaStream_t stream);
+int ms_deform_attn_bwd(const void* value, const float* proj, const float* ref, const void* d_out, float* d_value,
+                       float* d_proj, int N, int S_in, int Lq, int H, int D, int L, int P, int L_ref, const int* level_hw,
+                       const int* level_start, cudaStream_t stream);
 int ln_stats_finalize(const float* partial, int parts, int rows, int dim, float eps, float* mu, float* rstd,
                       cudaStream_t stream);
 

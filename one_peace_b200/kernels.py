@@ -3,6 +3,8 @@
 Every function takes CUDA tensors, passes raw device pointers + the current stream to
 ``libonepeace_b200.so`` and returns torch tensors.  Nothing here computes with torch ops.
 """
+import ctypes
+
 import torch
 
 from . import _lib
@@ -205,6 +207,61 @@ def attention_temporal_bwd(qkv, out, d_out, Bv, T, N, H, q_scale, dqkv=None):
     _lib.check(st, "opb_attention_temporal_bwd")
     _count()
     return dqkv
+
+
+def _msda_levels(shapes, starts):
+    L = len(shapes)
+    hw = (ctypes.c_int32 * (2 * L))(*[int(v) for s in shapes for v in s])
+    st = (ctypes.c_int32 * L)(*[int(v) for v in starts])
+    return hw, st
+
+
+def _msda_check(value, proj, ref, N, S_in, Lq, H, L, P):
+    assert value.dtype == torch.bfloat16 and value.shape == (N * S_in, H * 32) and value.is_contiguous()
+    assert proj.dtype == torch.float32 and proj.shape == (N * Lq, 3 * H * L * P) and proj.is_contiguous()
+    assert ref.dtype == torch.float32 and ref.dim() == 3 and ref.shape[0] == N * Lq and ref.shape[2] == 2 and ref.is_contiguous()
+
+
+def ms_deform_attn_fwd(value, proj, ref, shapes, starts, N, Lq, H, P, out=None):
+    """Multi-scale deformable attention core (include/onepeace_b200.h): value bf16 [N * S_in, H * 32], proj fp32
+    [N * Lq, 3 * H * L * P] (offsets | logits), ref fp32 [N * Lq, L_ref, 2], shapes [(H_l, W_l)] and starts host ints
+    -> out bf16 [N * Lq, H * 32]."""
+    _need_cuda(value, proj, ref, out)
+    L = len(shapes)
+    S_in = value.shape[0] // N
+    _msda_check(value, proj, ref, N, S_in, Lq, H, L, P)
+    if out is None:
+        out = torch.empty(N * Lq, H * 32, dtype=torch.bfloat16, device=value.device)
+    assert out.dtype == torch.bfloat16 and out.shape == (N * Lq, H * 32) and out.is_contiguous()
+    hw, st = _msda_levels(shapes, starts)
+    s = _lib.load().opb_ms_deform_attn_fwd(value.data_ptr(), proj.data_ptr(), ref.data_ptr(), out.data_ptr(), N, S_in, Lq, H,
+                                           32, L, P, ref.shape[1], hw, st, _stream())
+    _lib.check(s, "opb_ms_deform_attn_fwd")
+    _count()
+    return out
+
+
+def ms_deform_attn_bwd(value, proj, ref, d_out, shapes, starts, N, Lq, H, P, d_value=None, d_proj=None):
+    """Adjoint of ms_deform_attn_fwd for d_out bf16 [N * Lq, H * 32] -> (d_value fp32 [N * S_in, H * 32], accumulated into
+    (zeroed when not given), d_proj fp32 [N * Lq, 3 * H * L * P], overwritten)."""
+    _need_cuda(value, proj, ref, d_out, d_value, d_proj)
+    L = len(shapes)
+    S_in = value.shape[0] // N
+    _msda_check(value, proj, ref, N, S_in, Lq, H, L, P)
+    assert d_out.dtype == torch.bfloat16 and d_out.shape == (N * Lq, H * 32) and d_out.is_contiguous()
+    if d_value is None:
+        d_value = torch.zeros(value.shape, dtype=torch.float32, device=value.device)
+    if d_proj is None:
+        d_proj = torch.empty(proj.shape, dtype=torch.float32, device=value.device)
+    assert d_value.dtype == torch.float32 and d_value.shape == value.shape and d_value.is_contiguous()
+    assert d_proj.dtype == torch.float32 and d_proj.shape == proj.shape and d_proj.is_contiguous()
+    hw, st = _msda_levels(shapes, starts)
+    s = _lib.load().opb_ms_deform_attn_bwd(value.data_ptr(), proj.data_ptr(), ref.data_ptr(), d_out.data_ptr(),
+                                           d_value.data_ptr(), d_proj.data_ptr(), N, S_in, Lq, H, 32, L, P, ref.shape[1], hw,
+                                           st, _stream())
+    _lib.check(s, "opb_ms_deform_attn_bwd")
+    _count()
+    return d_value, d_proj
 
 
 def gemm_ln(a, w, epi, out, *, ln_mu=None, ln_rstd=None, ln_colsum=None, bias=None, colscale=None, gamma=None,
