@@ -25,7 +25,9 @@ A kernel output ``got`` passes ``assert_within`` when, element by element,
           (tiled, split-K, persistent) and is still 2^10 below the error of a wrong fragment row, a column slice shifted
           by 8 or a dropped k-block (tests/test_kernel_ref.py shows each of them failing).
 ``extra`` absolute allowances that do not scale with ``mag``: the fp32 evaluation of LayerNorm statistics from partial
-          records (``ln_stats_ref``) and, for the contrastive head, the errors of the bf16x3 logits.
+          records (``ln_stats_ref``), the fp32 colsum and bias of a LayerNorm fold when the reference takes their exact
+          values (``ln_colsum_err``, ``bias_err``: the ``ln_fold_ref`` bounds) and, for the contrastive head, the errors of
+          the bf16x3 logits.
 ``u_out`` 2^-8 for a bf16 output, 0 for fp32.  Round-to-nearest to 8 significant bits moves the kernel's fp32 value v by
           less than 2^-8 |v|, and |v| exceeds |ref| by at most the fp32 error (itself far inside tau * mag).
 
@@ -224,8 +226,12 @@ def ln_stats_ref(records, parts, M, dim, eps):
 
 def gemm_ref(a, w, epi, *, bias=None, colscale=None, gamma=None, resid=None, ln_mu=None, ln_rstd=None, ln_colsum=None,
              ln_partial=None, out_group=0, out_group_stride=0, out_row_offset=0, out_group_valid=0, resid_period=0,
-             resid_row_offset=0, stats=False):
+             resid_row_offset=0, stats=False, ln_colsum_err=None, bias_err=None):
     """fp64 result of ``epilogue(a[M,K] @ w[N,K]^T)`` as the kernel defines it (csrc/gemm.h), for the logical rows m < M.
+
+    ``ln_colsum_err`` / ``bias_err``: bounds of the fp32 colsum and bias the kernel reads when the given ``ln_colsum`` /
+    ``bias`` are the exact fp64 values of what ``ln_fold`` computed (``ln_fold_ref``).  The epilogue uses each once, so
+    the LN step gains rstd |mu| colsum_err and the bias step bias_err in ``extra``.
 
     Returns a namespace with
       y, mag, extra   [M, N_out] (N_out = N / 2 for GeGLU): the result and its bound terms (module docstring);
@@ -261,9 +267,13 @@ def gemm_ref(a, w, epi, *, bias=None, colscale=None, gamma=None, resid=None, ln_
         x = rstd * (x - mu * cs)
         xm = rstd * tm
         xe = rstd * (rel * tm + dmu * cs.abs())
+        if ln_colsum_err is not None:
+            xe = xe + rstd * mu.abs() * ln_colsum_err.double()[None, :]
     if bias is not None:
         x = x + bias.double()
         xm = xm + bias.double().abs()
+        if bias_err is not None:
+            xe = xe + bias_err.double()
     m = torch.arange(M, device=A.device)
     rows, valid = m, torch.ones(M, dtype=torch.bool, device=A.device)
     if out_group > 0:

@@ -23,9 +23,10 @@ tests/test_layer_ref.py), because the stack updates its gradient buffer and its 
             ->  [modality-major gather]  ->  dbqkv = colsum(dqkv), dWqkv = dqkv^T h1, dh1 = dqkv Wqkv
             ->  dx = dx2 + LN1'(x; dh1)
 The input x of layer i is the recorded output x3 of layer i - 1 (or, after the fused forward, the rows it kept for the
-recompute); dx3 of layer i is the recorded dx of layer i + 1 (or the upstream gradient).  The drop-path row scale rs is
-not read from any call: it is drawn again from the RNG state saved before the stack ran, as the stack draws it.  Row maps
-(parts, batch-major order) are rebuilt here from the part lengths.
+recompute, each checked to be the fused forward's recorded x after layer i - 1; the fused forward's own stages are those
+of tests/fused_ref.py); dx3 of layer i is the recorded dx of layer i + 1 (or the upstream gradient).  The drop-path row
+scale rs is not read from any call: it is drawn again from the RNG state saved before the stack ran, as the stack draws
+it.  Row maps (parts, batch-major order) are rebuilt here from the part lengths.
 
 Stack: the bias gradient of each table is ``dbias_ref`` over the dS of every (layer, sample) that used it, on zero (one
 launch per layer through the transposed table and its fold, or straight into the dense table), then ``center_ref`` when
@@ -35,6 +36,7 @@ from types import SimpleNamespace as NS
 
 import torch
 
+import fused_ref as FR
 import kernel_ref as R
 from stem_ref import b64
 
@@ -43,10 +45,11 @@ SHARED = ("q_w", "q_b", "k_w", "v_w", "v_b", "o_w", "o_b", "lni_w", "lni_b", "ln
           "g2")
 FFN = ("wi0", "wi1", "lnf_w", "lnf_b", "w2", "b2")
 # outputs that are column reductions (sums over rows: bias, LayerNorm and LayerScale gradients, the bias tables) and
-# outputs that are exact row copies (y: the stack output is the last layer's x3)
+# outputs that are exact row copies (y: the stack output is the last layer's x3; kept: the layer inputs the fused forward
+# kept)
 REDUCTIONS = ("q_b", "v_b", "o_b", "lni_w", "lni_b", "ln1_w", "ln1_b", "ln2_w", "ln2_b", "g1", "g2", "lnf_w", "lnf_b", "b2",
               "db2", "dbias")
-EXACT = ("qkv_bm", "att_mm", "datt_bm", "dqkv_mm", "y")
+EXACT = ("qkv_bm", "att_mm", "datt_bm", "dqkv_mm", "y", "kept")
 
 
 def is_reduction(name):
@@ -404,10 +407,12 @@ def bias_grad_refs(biases, brs, shared_tables, S):
 def stack_checks(encoder, lay, x0, dy, y, biases, key_pad, rs, fwd_log, bwd_log, shared_tables, kept_inputs=None):
     """every check of one EncoderStackFn forward and backward.  fwd_log / bwd_log: ``Snapshots`` entries of the forward
     and of the backward; biases: the stack's bias inputs (leaves whose .grad is checked); rs: ``row_scales``;
-    kept_inputs: the layer inputs the fused forward kept for the recompute (None when the forward ran layer by layer).
+    kept_inputs: the layer inputs the fused forward kept for the recompute (None when the forward ran layer by layer; the
+    fused forward's calls are then checked from fwd_log by ``fused_ref.encoder_checks``).
     Returns (checks, got) for ``stem_ref.shares``."""
     layers = list(encoder.layers)
     L, d = len(layers), x0.shape[-1]
+    chk, got = {}, {}
     fw = [parse_fwd(c, lay) for k, c in segments(fwd_log, lay) if k == "fwd"]
     seg = segments(bwd_log, lay)
     recompute = [parse_fwd(c, lay) for k, c in seg if k == "fwd"]
@@ -419,8 +424,17 @@ def stack_checks(encoder, lay, x0, dy, y, biases, key_pad, rs, fwd_log, bwd_log,
     logical = [None if b is None else (b[0] if b.dim() == 4 and b.shape[0] == 1 else b)[..., :lay.S].detach()
                for b in bias_i]
     transposed = bw[0].transposed
+    if not fw:
+        # the fused-LayerNorm forward: its stages from its own log (fused_ref), each kept input the recorded x after the
+        # layer below (exactly), the output the last recorded x
+        chk, got, xs = FR.encoder_checks(encoder, x0.detach().reshape(-1, d), logical if biases else [], key_pad, lay.B,
+                                         lay.S, lay.parts[0][0], fwd_log)
+        for i, t in enumerate(kept_inputs):
+            ref = (x0.detach().reshape(-1, d) if i == 0 else xs[i - 1]).double()
+            chk[f"L{i}.kept"], got[f"L{i}.kept"] = (ref, torch.zeros_like(ref), F32), t
+        chk["y"] = (xs[-1].double(), torch.zeros_like(xs[-1], dtype=torch.float64), F32)
+        got["y"] = y.detach().reshape(-1, d)
     X = [x0.detach().reshape(-1, d)] + ([f.x3 for f in fw[:-1]] if fw else [t for t in kept_inputs[1:]])
-    chk, got = {}, {}
 
     def add(prefix, c, g):
         for k in c:

@@ -15,11 +15,13 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+import det_ref as D
 import kernel_ref as R
 import stem_ref as SR
 import test_classify_host_logic as CH
 from grounding_ref import refcoco
 from one_peace_b200 import autograd as AG
+from one_peace_b200.kernels import RelPosBias
 from vit_ref import head_bwd, head_fwd
 
 BF = torch.bfloat16
@@ -35,6 +37,7 @@ class Emu:
     that share a table keep only the last one's).  tests/test_layer_ref.py runs the encoder stack on it."""
     EPI_STORE_BF16, EPI_GEGLU_BF16, EPI_RESID_F32, EPI_STORE_F32, EPI_GELU_BF16 = 0, 1, 2, 3, 4
     BIAS_T_KEYS, BIAS_T_Q = 256, 224        # the transposed bias tables of the attention backward
+    RelPosBias = RelPosBias                 # the bias container, as kernels.RelPosBias
 
     def __init__(self, **flags):
         self.text_pad_grad = flags.pop("text_pad_grad", False)
@@ -56,6 +59,8 @@ class Emu:
             y = y + bias.double()
         if colscale is not None:
             y = y * colscale.double()
+        if epi == self.EPI_GELU_BF16:
+            y = F.gelu(y)
         if epi == self.EPI_RESID_F32:
             N = y.shape[1]
             m = torch.arange(y.shape[0])
@@ -198,7 +203,32 @@ class Emu:
 
     def row_stats_cast(self, x, out_bf16, mu, rstd, eps=1e-5):
         out_bf16.copy_(x.to(BF))
+        r = R.layernorm_ref(x, None, None, eps)
+        mu.copy_(r.mu)
+        rstd.copy_(r.rstd)
         return out_bf16
+
+    # the fused-LayerNorm layer loops (TransformerEncoder.run_fused, VideoLayer.forward_video): the GEMM with its LayerNorm
+    # fold, records and bf16 side output (csrc/gemm.h) and the fold itself (csrc/pack.cu), on their fp64 references
+    def gemm_ln(self, a, w, epi, out, *, ln_partial=None, stats_out=None, out_bf16=None, workspace=None, cta_group=0, **kw):
+        M, N = a.shape[0], out.shape[-1]
+        if ln_partial is not None:                          # the kernel reads the first `parts` records of every row
+            rec, parts, dim, eps = ln_partial
+            ln_partial = (rec.reshape(-1)[:parts * M * 2], parts, dim, eps)
+        g = R.gemm_ref(a, w, epi, ln_partial=ln_partial, stats=stats_out is not None, **kw)
+        o = out.view(-1, N)
+        o[g.rows[g.valid]] = g.y[g.valid].to(out.dtype)
+        if out_bf16 is not None:
+            out_bf16.view(-1, N)[g.rows[g.valid]] = o[g.rows[g.valid]].to(BF)
+        if stats_out is not None:
+            stats_out.view(-1)[:g.stats.numel()] = g.stats.reshape(-1).float()
+        return out
+
+    def ln_fold(self, weight, ln_w, ln_b, bias, out_w, colsum, bias_out, interleave=0):
+        r = R.ln_fold_ref(weight, ln_w, ln_b, bias, interleave)
+        out_w[r.rows] = r.wg
+        colsum[r.rows] = r.colsum.float()
+        bias_out[r.rows] = r.bias.float()
 
     def window_gather(self, x, B, t_in, t_out, stride, kw, pad, groups):
         cg = x.shape[1] // groups
@@ -287,17 +317,46 @@ class Emu:
 
     # the encoder stack's attention (csrc/attention.cu, attention_bwd.cu): the fp64 references on the values the kernels read
     def attention(self, qkv, bias, key_pad, B, S, H, out=None, lse=None, ln_stats=None):
-        assert ln_stats is None
         f = R.attention_ref(qkv, None if bias is None else bias[..., :S], key_pad, B, S, H)
         out.copy_(f.out)
         if lse is not None:
             lse.copy_(f.lse.reshape(-1))
+        if ln_stats is not None:                            # [H, B S, 2] of the fp32 rows before rounding
+            ln_stats.view(-1).copy_(f.stats.reshape(-1))
         return out
 
     def attention_tc(self, qkv, rp, key_pad, B, S, H, out=None, ln_stats=None, lse=None):
         assert not getattr(rp, "seg_split", 0)
         dense = rp.lut[:, (rp.code_row[:S, None] - rp.code_col[None, :S]).long()]
         return self.attention(qkv, dense, key_pad, B, S, H, out=out, lse=lse, ln_stats=ln_stats)
+
+    def relpos_decomp_proj(self, qkv, rel_pos_h, rel_pos_w, pos_y, pos_x, B, S, H, kh, kw, q_unscale=8.0, rel_h=None,
+                           rel_w=None):
+        rh, _, rw, _ = D.proj_ref(qkv, rel_pos_h, rel_pos_w, pos_y, pos_x, B, S, H, kh, kw)
+        s = q_unscale / D.Q_UNSCALE                         # proj_ref multiplies q by the model's unscale
+        return (rh * s).float(), (rw * s).float()
+
+    def attention_decomp(self, qkv, rp, rel_h, rel_w, key_y, key_x, B, S, H, kh, kw, out=None, ln_stats=None, lse=None):
+        dense = rp.lut[:, (rp.code_row[:S, None] - rp.code_col[None, :S]).long()]
+        f = D.decomp_attention_ref(qkv, dense, rel_h, torch.zeros_like(rel_h), rel_w, torch.zeros_like(rel_w), key_y, key_x,
+                                   B, S, H)
+        out.copy_(f.out)
+        if lse is not None:
+            lse.copy_(f.lse.reshape(-1))
+        if ln_stats is not None:
+            ln_stats.view(-1).copy_(f.stats.reshape(-1))
+        return out
+
+    def attention_temporal(self, qkv, Bv, T, N, H, out=None, ln_stats=None):
+        b, n, t = torch.meshgrid(torch.arange(Bv), torch.arange(N), torch.arange(T), indexing="ij")
+        idx = ((b * T + t) * N + n).reshape(-1)               # sequence b N + n: the T frames of token n of clip b
+        f = R.attention_ref(qkv[idx], None, None, Bv * N, T, H)
+        out[idx] = f.out.to(out.dtype)
+        ln_stats.view(H, -1, 2)[:, idx] = f.stats.float()
+        return out, ln_stats
+
+    def relpos_lut_build(self, table, idx):
+        return R.relpos_lut_ref(table, idx).contiguous()
 
     def attention_bwd(self, qkv, out, d_out, bias, key_pad, lse, dqkv, dbias, B, S, H, q_scale):
         r = R.attention_bwd_ref(qkv, out, d_out, lse, None if bias is None else bias[..., :S], key_pad, B, S, H, q_scale)
