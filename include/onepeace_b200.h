@@ -193,6 +193,31 @@ int opb_ms_deform_attn_bwd(const void* value, const float* proj, const float* re
                            const int32_t* level_hw, const int32_t* level_start, void* stream);
 
 /*
+ * Segmentation backbone (one_peace_vision/seg, OnePeaceAdapter).
+ *   opb_seg_dwconv_gelu : ConvFFN's depthwise conv (adapter_modules.py:69-84) + bias + exact GELU over token rows.
+ *     x, y bf16 [B * T, C], T = sum_l H_l W_l; each sample's rows hold the n_levels levels back to back, level l a row-major
+ *     H_l x W_l grid (level_hw [n_levels, 2] = (H_l, W_l), a HOST int32 array passed by value).  Each level is convolved on
+ *     its own grid with zero padding at its border:  y = gelu_erf(sum_{ky, kx} x[tap] * w[ky * 3 + kx, c] + bias[c]), fp32
+ *     products summed in tap order.  w fp32 [9, C] (the conv weight [C, 1, 3, 3] rearranged tap-major), bias fp32 [C].
+ *     No atomics: repeats are bit-identical.  Needs B >= 1, C % 8 == 0, 1 <= n_levels <= 4, positive level sides and
+ *     non-null 16-byte aligned pointers, else OPB_ERR_INVALID before a launch.
+ *   opb_seg_out_map : one output map of onepeace_adapter.py:114-134, fp32 NCHW out [B, C, Hl, Wl]:
+ *       out[b, c, y, x] = scale[c] * (extra[b, y, x, c] + c_l[b, y, x, c] + up[b, c, y, x]) + shift[c]
+ *     c_l : fp32 rows, pixel (y, x) of sample b at row b * c_sample_rows + c_row0 + y * Wl + x, C wide.
+ *     up  : the bilinear resize (align_corners = False, scale gw / Hl and gw / Wl) of the gw x gw grid of fp32 rows
+ *           b * x_sample_rows + x_row0 + i * gw + j of x.
+ *     extra : NULL, or fp32 [B * (Hl / 2) * (Wl / 2), 4 * C], the transposed conv (k = s = 2) as one GEMM with columns
+ *           (dy, dx, c): pixel (y, x) reads row (b, y / 2, x / 2), column ((y % 2) * 2 + x % 2) * C + c.
+ *     scale / shift fp32 [C]: the eval BatchNorm folded.  C % 32 == 0, rows inside their samples, even Hl and Wl with
+ *     extra, else OPB_ERR_INVALID before a launch.
+ */
+int opb_seg_dwconv_gelu(const void* x, const float* w, const float* bias, void* y, int B, int C, int n_levels,
+                        const int32_t* level_hw, void* stream);
+int opb_seg_out_map(const float* c, int64_t c_sample_rows, int64_t c_row0, const float* x, int64_t x_sample_rows,
+                    int64_t x_row0, int gw, const float* extra, const float* scale, const float* shift, float* out, int B,
+                    int C, int Hl, int Wl, void* stream);
+
+/*
  * GEMM with the full epilogue description (superset of opb_gemm_bf16).  Adds the fused-LayerNorm form
  *   LN(x) W^T + b  =  rstd[m] * (acc - mu[m] * colsum[n]) + bias'[n]
  * where A holds the UN-normalised rows (bf16), B = W * diag(ln_weight) (bf16), colsum[n] = sum_k B[n,k],

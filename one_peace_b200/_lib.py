@@ -40,6 +40,9 @@ SIGNATURES = {
                                        c_int, c_int, c_void_p, c_void_p, c_void_p]),
     "opb_ms_deform_attn_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int,
                                        c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
+    "opb_seg_dwconv_gelu": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
+    "opb_seg_out_map": (c_int, [c_void_p, c_int64, c_int64, c_void_p, c_int64, c_int64, c_int, c_void_p, c_void_p, c_void_p,
+                                c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
     "opb_gemm_bf16_ex": (c_int, [c_void_p, c_void_p]),
     "opb_row_stats_cast": (c_int, [c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_void_p, c_int, c_int, c_float, c_void_p]),
     "opb_ln_stats_finalize": (c_int, [c_void_p, c_int, c_int, c_int, c_float, c_void_p, c_void_p, c_void_p]),

@@ -81,6 +81,18 @@ int opb_ms_deform_attn_bwd(const void* value, const float* proj, const float* re
                                  level_start, static_cast<cudaStream_t>(stream));
 }
 
+int opb_seg_dwconv_gelu(const void* x, const float* w, const float* bias, void* y, int B, int C, int n_levels,
+                        const int32_t* level_hw, void* stream) {
+  return opb::seg_dwconv_gelu(x, w, bias, y, B, C, n_levels, level_hw, static_cast<cudaStream_t>(stream));
+}
+
+int opb_seg_out_map(const float* c, int64_t c_sample_rows, int64_t c_row0, const float* x, int64_t x_sample_rows,
+                    int64_t x_row0, int gw, const float* extra, const float* scale, const float* shift, float* out, int B,
+                    int C, int Hl, int Wl, void* stream) {
+  return opb::seg_out_map(c, c_sample_rows, c_row0, x, x_sample_rows, x_row0, gw, extra, scale, shift, out, B, C, Hl, Wl,
+                          static_cast<cudaStream_t>(stream));
+}
+
 int opb_relpos_lut_build(const float* table, const int32_t* idx, float* lut, int L, int H, void* stream) {
   if (!table || !idx || !lut) return OPB_ERR_INVALID;
   return opb::relpos_lut_build(table, idx, lut, L, H, static_cast<cudaStream_t>(stream));

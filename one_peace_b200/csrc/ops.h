@@ -59,6 +59,14 @@ int ms_deform_attn_fwd(const void* value, const float* proj, const float* ref, v
 int ms_deform_attn_bwd(const void* value, const float* proj, const float* ref, const void* d_out, float* d_value,
                        float* d_proj, int N, int S_in, int Lq, int H, int D, int L, int P, int L_ref, const int* level_hw,
                        const int* level_start, cudaStream_t stream);
+// Segmentation backbone (csrc/seg.cu): ConvFFN's per-level depthwise 3x3 conv + bias + GELU over token rows, and one
+// output map (residual sum, bilinear ViT term, optional pixel-shuffled transposed conv, folded BatchNorm) to fp32 NCHW.
+constexpr int kSegMaxL = 4;
+int seg_dwconv_gelu(const void* x, const float* w, const float* bias, void* y, int B, int C, int n_levels,
+                    const int* level_hw, cudaStream_t stream);
+int seg_out_map(const float* c, long c_sample_rows, long c_row0, const float* x, long x_sample_rows, long x_row0, int gw,
+                const float* extra, const float* scale, const float* shift, float* out, int B, int C, int Hl, int Wl,
+                cudaStream_t stream);
 int ln_stats_finalize(const float* partial, int parts, int rows, int dim, float eps, float* mu, float* rstd,
                       cudaStream_t stream);
 

@@ -264,6 +264,49 @@ def ms_deform_attn_bwd(value, proj, ref, d_out, shapes, starts, N, Lq, H, P, d_v
     return d_value, d_proj
 
 
+def seg_dwconv_gelu(x, w, bias, level_shapes, B, out=None):
+    """ConvFFN's per-level depthwise 3x3 conv + bias + exact GELU (include/onepeace_b200.h): x bf16 [B * T, C] with each
+    sample's T = sum H_l W_l rows holding the levels level_shapes [(H_l, W_l)] back to back, w fp32 [9, C] tap-major, bias
+    fp32 [C] -> out bf16 [B * T, C]."""
+    _need_cuda(x, w, bias, out)
+    C = x.shape[1]
+    assert x.dtype == torch.bfloat16 and x.is_contiguous() and x.shape[0] == B * sum(h * v for h, v in level_shapes)
+    assert w.dtype == torch.float32 and w.shape == (9, C) and w.is_contiguous()
+    assert bias.dtype == torch.float32 and bias.shape == (C,) and bias.is_contiguous()
+    if out is None:
+        out = torch.empty_like(x)
+    assert out.dtype == torch.bfloat16 and out.shape == x.shape and out.is_contiguous()
+    hw = (ctypes.c_int32 * (2 * len(level_shapes)))(*[int(v) for s in level_shapes for v in s])
+    st = _lib.load().opb_seg_dwconv_gelu(x.data_ptr(), w.data_ptr(), bias.data_ptr(), out.data_ptr(), B, C,
+                                         len(level_shapes), hw, _stream())
+    _lib.check(st, "opb_seg_dwconv_gelu")
+    _count()
+    return out
+
+
+def seg_out_map(c, c_sample_rows, c_row0, x, x_sample_rows, x_row0, gw, scale, shift, B, Hl, Wl, extra=None, out=None):
+    """One segmentation output map (include/onepeace_b200.h): out fp32 [B, C, Hl, Wl] = scale * (extra + c_l + bilinear
+    resize of the gw x gw ViT grid) + shift, from the token-major fp32 rows of c and x at the given per-sample row strides
+    and offsets; extra: None or the transposed conv's fp32 [B * Hl / 2 * Wl / 2, 4 C] GEMM output."""
+    _need_cuda(c, x, scale, shift, extra, out)
+    C = c.shape[-1]
+    for t in (c, x, extra):
+        assert t is None or (t.dtype == torch.float32 and t.is_contiguous())
+    assert x.shape[-1] == C and c.numel() >= B * c_sample_rows * C and x.numel() >= B * x_sample_rows * C
+    assert extra is None or extra.shape == (B * (Hl // 2) * (Wl // 2), 4 * C)
+    for t in (scale, shift):
+        assert t.dtype == torch.float32 and t.shape == (C,) and t.is_contiguous()
+    if out is None:
+        out = torch.empty(B, C, Hl, Wl, dtype=torch.float32, device=c.device)
+    assert out.dtype == torch.float32 and out.shape == (B, C, Hl, Wl) and out.is_contiguous()
+    st = _lib.load().opb_seg_out_map(c.data_ptr(), c_sample_rows, c_row0, x.data_ptr(), x_sample_rows, x_row0, gw,
+                                     _ptr(extra), scale.data_ptr(), shift.data_ptr(), out.data_ptr(), B, C, Hl, Wl,
+                                     _stream())
+    _lib.check(st, "opb_seg_out_map")
+    _count()
+    return out
+
+
 def gemm_ln(a, w, epi, out, *, ln_mu=None, ln_rstd=None, ln_colsum=None, bias=None, colscale=None, gamma=None,
             resid=None, stats_out=None, out_bf16=None, cta_group=0, workspace=None, ln_partial=None, out_group=0,
             out_group_stride=0, out_row_offset=0, out_group_valid=0, resid_period=0, resid_row_offset=0):

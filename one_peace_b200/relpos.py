@@ -70,10 +70,7 @@ class LutCache:
         key = (S, str(device))
         if key not in self._c:
             b = bucket_tensor[:S, :S].detach().cpu().numpy()
-            r = build_lut_index(b, codes_fn(S))
-            if r is not None and (r[0].size * 4 + ((S + 3) // 4) * 4 * 4 + S + 64) > 40 * 1024:
-                r = None                      # would not fit the kernel's table region (csrc/attention_tc.cu: 13 KB inside the dead
-                                              # Q tile, up to 40 KB in a region of its own for long sequences)
+            r = build_lut_index(b, codes_fn(S))      # any length: a LUT too long to stage is read from global memory
             self._c[key] = None if r is None else tuple(torch.from_numpy(a).to(device) for a in r)
         return self._c[key]
 

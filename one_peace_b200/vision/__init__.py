@@ -1,6 +1,6 @@
 """The vision branch's backbones: the ImageNet classifier (one_peace_vision/classification: ``models_vit`` and the criteria
-of ``main_ft.py``), the detection backbone (``det``), the action-recognition backbone (``video``) and the segmentation
-recipe's multi-scale deformable attention (``ms_deform_attn.MSDeformAttn``)."""
+of ``main_ft.py``), the detection backbone (``det``), the action-recognition backbone (``video``), the segmentation
+backbone (``seg``) and its multi-scale deformable attention (``ms_deform_attn.MSDeformAttn``)."""
 import torch
 import torch.nn.functional as F
 

@@ -71,6 +71,22 @@ def msda_pack(m, cache):
     return cache.get(ps, build)
 
 
+def msda_forward(pk, q, x, ref, shapes, starts, N, Lq, H, P, out, epi, **epilogue):
+    """value_proj, the fused offset / logit projection, the core and output_proj: q bf16 [N * Lq, d], x bf16 [N * S_in, d]
+    -> (value, proj, core).  output_proj writes `out` through epilogue `epi` with bias bo and the GEMM options `epilogue`
+    (e.g. the in-place residual of the segmentation backbone's injectors and extractors)."""
+    dev = q.device
+    value = K.gemm(x, pk["wv"], K.EPI_STORE_BF16, torch.empty(x.shape[0], pk["wv"].shape[0], dtype=torch.bfloat16, device=dev),
+                   bias=pk["bv"])
+    proj = K.gemm(q, pk["wp"], K.EPI_STORE_F32, torch.empty(N * Lq, pk["wp"].shape[0], dtype=torch.float32, device=dev),
+                  bias=pk["bp"])
+    if proj.shape[1] != pk["n_proj"]:
+        proj = proj[:, :pk["n_proj"]].contiguous()
+    core = K.ms_deform_attn_fwd(value, proj, ref, shapes, starts, N, Lq, H, P)
+    K.gemm(core, pk["wo"], epi, out, bias=pk["bo"], **epilogue)
+    return value, proj, core
+
+
 class MSDeformAttnFn(torch.autograd.Function):
     """(query [N, Lq, d], input_flatten [N, S_in, d]) -> output [N, Lq, d] in the query's dtype.  meta = (pack, reference
     points fp32 [N * Lq, L_ref, 2], level shapes, start rows, n_heads, n_points); then the eight msda_params."""
@@ -83,15 +99,8 @@ class MSDeformAttnFn(torch.autograd.Function):
         dev = query.device
         q = query.reshape(N * Lq, d).to(torch.bfloat16).contiguous()
         x = input_flatten.reshape(N * S_in, d).to(torch.bfloat16).contiguous()
-        dv = pk["wv"].shape[0]
-        value = K.gemm(x, pk["wv"], K.EPI_STORE_BF16, torch.empty(N * S_in, dv, dtype=torch.bfloat16, device=dev),
-                       bias=pk["bv"])
-        proj = K.gemm(q, pk["wp"], K.EPI_STORE_F32, torch.empty(N * Lq, pk["wp"].shape[0], dtype=torch.float32, device=dev),
-                      bias=pk["bp"])
-        if proj.shape[1] != pk["n_proj"]:
-            proj = proj[:, :pk["n_proj"]].contiguous()
-        core = K.ms_deform_attn_fwd(value, proj, ref, shapes, starts, N, Lq, H, P)
-        y = K.gemm(core, pk["wo"], K.EPI_STORE_F32, torch.empty(N * Lq, d, dtype=torch.float32, device=dev), bias=pk["bo"])
+        y = torch.empty(N * Lq, d, dtype=torch.float32, device=dev)
+        value, proj, core = msda_forward(pk, q, x, ref, shapes, starts, N, Lq, H, P, y, K.EPI_STORE_F32)
         ctx.meta = (pk, ref, shapes, starts, H, P, N, Lq, S_in, d)
         ctx.saved = (q, x, value, proj, core)
         ctx.dtypes = [p.dtype for p in params]
